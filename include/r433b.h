@@ -269,7 +269,7 @@ int r433b_pulses_load_rfraw(r433b_pulses *ps, uint32_t stream, char const *line)
 int r433b_pulses_add(r433b_pulses *ps, uint32_t stream, struct pulse_data const *pd);
 uint32_t r433b_pulses_count(r433b_pulses const *ps);
 int r433b_pulses_get(r433b_pulses const *ps, uint32_t index, struct pulse_data *out);
-/* All slicers of the registered devices on every package of the set (k_slice only). */
+/* All slicers of the registered devices on every package of the set (the slicer stage only: no IQ, no detector). */
 int r433b_process_pulses(r433b_ctx *ctx, r433b_pulses const *ps);
 
 /* Writers; all return the length of the full text (snprintf convention), writing at most cap bytes.

@@ -1,6 +1,6 @@
 // r433b_api.cu -- the C ABI declared in include/r433b.h: context, batch processing on the GPU,
 // result fetch, and the CPU-side replay that feeds events to decoders in the reference's order.
-// There is no CPU implementation of the DSP here: every sample goes through k_detect/k_slice.
+// There is no CPU implementation of the DSP here: every sample goes through k_detect/k_slice2.
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
@@ -67,10 +67,7 @@ struct r433b_ctx {
     unsigned fpdm = 0;
     int enable_fm = 0;
     int n_sms = 132;        // cudaDevAttrMultiProcessorCount of `device`
-    unsigned stage_words = kStageWords; // R433B_STAGE_WORDS overrides (tuning experiments)
     int spoil_front = 0; // R433B_SPOIL_FRONT=1|2: k_front starts from wrong guesses (tests of the redo / repair paths)
-    int slice_v2 = 1; // k_slice2 (lanes = packages of one device); R433B_SLICE_V1=1 selects k_slice (lanes = devices on one package)
-    int lazy_fm = 1; // R433B_EAGER_FM=1 in the environment turns the on-demand FM path off (A/B checks)
     Levels lv{};
     // device memory (grow only)
     DevBuf d_data, d_offsets, d_train, d_pkgs, d_ppool, d_gpool, d_counters, d_am, d_fm;
@@ -206,10 +203,7 @@ int r433b_create(int cuda_device, r433b_ctx **out)
     for (auto &v : ctx->ev_f) cudaEventCreate(&v);
     cudaEventCreateWithFlags(&ctx->ev_init, cudaEventDisableTiming);
     ctx->lv = compute_levels(0, 0.0f, -12.1442f, 9.0f);
-    if (char const *v = getenv("R433B_EAGER_FM")) ctx->lazy_fm = !(v[0] && v[0] != '0');
-    if (char const *v = getenv("R433B_SLICE_V1")) ctx->slice_v2 = !(v[0] && v[0] != '0');
     if (char const *v = getenv("R433B_SPOIL_FRONT")) ctx->spoil_front = atoi(v);
-    if (char const *v = getenv("R433B_STAGE_WORDS")) ctx->stage_words = (unsigned)std::max(8, atoi(v));
     if (cudaDeviceGetAttribute(&ctx->n_sms, cudaDevAttrMultiProcessorCount, cuda_device) != cudaSuccess || ctx->n_sms <= 0)
         ctx->n_sms = 132;
     *out = ctx;
@@ -313,21 +307,102 @@ int r433b_set_r_devices(r433b_ctx *ctx, struct r_device *const *devs, uint32_t n
 
 namespace {
 
-// The slicers over one package range: k_bucket + k_slice2 (lanes = packages of one device), or k_slice.
-void launch_slice(r433b_ctx *ctx, SliceParams const &q, unsigned slice_grid, cudaStream_t st)
+// The slicer tables of a batch: every device scaled to each sample rate of `rates` (with its gate; the package
+// range of rate g reads entries [g * n_devs, (g + 1) * n_devs)) and the OOK / FSK device lists.  Also sizes
+// k_slice2's staging scratch: the kernel runs as a fixed grid whose warps fetch work items (GroupRange::next), and
+// every thread of that grid owns kStageWords of scratch for the staged single pass.
+int upload_slicer_tables(r433b_ctx *ctx, std::vector<uint32_t> const &rates, cudaStream_t st)
 {
-    if (ctx->slice_v2) {
-        Slice2Params q2{};
-        q2.s = q;
-        q2.order = (unsigned const *)ctx->d_order.p;
-        unsigned const bgrid = (unsigned)ctx->n_sms * 2;
-        R4_LAUNCH(k_bucket_count, bgrid, kBucketThreads, 0, st, q.range, q.pkgs, q.n_pkgs, q.n_devs);
-        R4_LAUNCH(k_bucket_scan, 1, 1, 0, st, q.range);
-        R4_LAUNCH(k_bucket_scatter, bgrid, kBucketThreads, 0, st, q.range, (r433b_package const *)q.pkgs, q.n_pkgs, (unsigned *)ctx->d_order.p);
-        R4_LAUNCH(k_slice2, slice_grid, kSliceThreads, 0, st, q2);
-    } else {
-        R4_LAUNCH(k_slice, slice_grid, kSliceThreads, 0, st, q);
+    size_t const n_devs = ctx->devs.size();
+    std::vector<SlicerParams> sp(rates.size() * n_devs);
+    for (size_t g = 0; g < rates.size(); ++g)
+        for (size_t i = 0; i < n_devs; ++i) {
+            sp[g * n_devs + i] = scale_device(ctx->devs[i], rates[g]);
+            if (!ctx->gates.empty()) sp[g * n_devs + i].gate = ctx->gates[i].min_bits;
+        }
+    std::vector<unsigned> lists = slice_list(ctx->devs, 1), fsk = slice_list(ctx->devs, 2);
+    ctx->n_ook = (unsigned)lists.size();
+    ctx->n_fsk = (unsigned)fsk.size();
+    lists.insert(lists.end(), fsk.begin(), fsk.end());
+    if (int r = dev_reserve(ctx, ctx->d_devparams, std::max<size_t>(1, sp.size()) * sizeof(SlicerParams))) return r;
+    if (int r = dev_reserve(ctx, ctx->d_lists, (lists.size() + 1) * sizeof(unsigned))) return r;
+    size_t const stage_threads = (size_t)ctx->n_sms * kSliceCtasPerSm * kSliceThreads;
+    if (int r = dev_reserve(ctx, ctx->d_stage, stage_threads * kStageWords * sizeof(uint32_t))) return r;
+    if (!sp.empty()) CU(cudaMemcpyAsync(ctx->d_devparams.p, sp.data(), sp.size() * sizeof(SlicerParams), cudaMemcpyHostToDevice, st));
+    if (!lists.empty()) CU(cudaMemcpyAsync(ctx->d_lists.p, lists.data(), lists.size() * sizeof(unsigned), cudaMemcpyHostToDevice, st));
+    return R433B_OK;
+}
+
+// The slicers over one package range: k_bucket sorts its packages, k_slice2 runs every slicer on them with the
+// tables of sample rate `rate_index`.  `n_pkgs` bounds the range, whose end may only be known on the device.
+void launch_slice(r433b_ctx *ctx, GroupRange *range, unsigned n_pkgs, unsigned rate_index, cudaStream_t st)
+{
+    unsigned const n_devs = (unsigned)ctx->devs.size();
+    r433b_package *pkgs = (r433b_package *)ctx->d_pkgs.p;
+    SliceParams q{};
+    q.pkgs = pkgs;
+    q.range = range;
+    q.order = (unsigned const *)ctx->d_order.p;
+    q.pulse_pool = (int const *)ctx->d_ppool.p;
+    q.gap_pool = (int const *)ctx->d_gpool.p;
+    q.dev = (SlicerParams const *)ctx->d_devparams.p + (size_t)rate_index * n_devs;
+    q.n_devs = n_devs;
+    q.ook_list = (unsigned const *)ctx->d_lists.p;
+    q.fsk_list = q.ook_list + ctx->n_ook;
+    q.n_ook = ctx->n_ook;
+    q.n_fsk = ctx->n_fsk;
+    q.pairs = (r433b_pair *)ctx->d_pairs.p;
+    q.arena = (uint8_t *)ctx->d_arena.p;
+    q.arena_cap = ctx->arena_cap;
+    q.cursor = (unsigned long long *)ctx->d_cursor.p;
+    q.stage = (uint32_t *)ctx->d_stage.p;
+    q.stage_words = kStageWords;
+    unsigned const bgrid = (unsigned)ctx->n_sms * 2;
+    R4_LAUNCH(k_bucket_count, bgrid, kBucketThreads, 0, st, range, pkgs, n_pkgs, n_devs);
+    R4_LAUNCH(k_bucket_scan, 1, 1, 0, st, range);
+    R4_LAUNCH(k_bucket_scatter, bgrid, kBucketThreads, 0, st, range, (r433b_package const *)pkgs, n_pkgs, (unsigned *)ctx->d_order.p);
+    R4_LAUNCH(k_slice2, (unsigned)ctx->n_sms * kSliceCtasPerSm, kSliceThreads, 0, st, q);
+}
+
+// The slicer stage over package ranges known on the host: range g (pkg_begin / pkg_end set, the rest zero) uses
+// slicer table g.  Runs again with an event arena grown to what the device counted until every event fits, times
+// the stage with ev[2] -> ev[3] and leaves the event totals in the context.
+int slice_ranges(r433b_ctx *ctx, std::vector<GroupRange> const &ranges, unsigned n_pkgs, cudaStream_t st)
+{
+    unsigned const n_devs = (unsigned)ctx->devs.size();
+    unsigned long long cursor[4] = {0, 0, 0, 0};
+    ctx->timing.slice_launches = 0;
+    CU(cudaEventRecord(ctx->ev[2], st));
+    if (n_pkgs && n_devs) {
+        size_t const pair_bytes = (size_t)n_pkgs * n_devs * sizeof(r433b_pair);
+        if (int r = dev_reserve(ctx, ctx->d_pairs, pair_bytes)) return r;
+        if (int r = dev_reserve(ctx, ctx->d_order, (size_t)n_pkgs * sizeof(unsigned))) return r;
+        if (int r = dev_reserve(ctx, ctx->d_ranges, ranges.size() * sizeof(GroupRange))) return r;
+        if (int r = dev_reserve(ctx, ctx->d_cursor, 64)) return r;
+        for (int attempt = 0; attempt < 3; ++attempt) {
+            if (int r = dev_reserve(ctx, ctx->d_arena, ctx->arena_cap)) return r;
+            CU(cudaMemsetAsync(ctx->d_pairs.p, 0, pair_bytes, st));
+            CU(cudaMemsetAsync(ctx->d_cursor.p, 0, 64, st));
+            CU(cudaMemcpyAsync(ctx->d_ranges.p, ranges.data(), ranges.size() * sizeof(GroupRange), cudaMemcpyHostToDevice, st));
+            for (size_t g = 0; g < ranges.size(); ++g) {
+                launch_slice(ctx, (GroupRange *)ctx->d_ranges.p + g, n_pkgs, (unsigned)g, st);
+                CU(cudaGetLastError());
+                ctx->timing.slice_launches++;
+            }
+            CU(cudaMemcpyAsync(cursor, ctx->d_cursor.p, sizeof(cursor), cudaMemcpyDeviceToHost, st));
+            CU(cudaStreamSynchronize(st));
+            if (!cursor[2]) break;
+            ctx->arena_cap = (size_t)cursor[0] + (1u << 20);
+            if (attempt == 2) return fail(ctx, R433B_EOVERFLOW, "event arena overflow");
+        }
     }
+    CU(cudaEventRecord(ctx->ev[3], st));
+    CU(cudaEventSynchronize(ctx->ev[3]));
+    cudaEventElapsedTime(&ctx->timing.slice_ms, ctx->ev[2], ctx->ev[3]);
+    ctx->event_bytes = cursor[0];
+    ctx->n_events = cursor[1];
+    ctx->n_gated = cursor[3];
+    return R433B_OK;
 }
 
 } // namespace
@@ -428,7 +503,6 @@ int r433b_process(r433b_ctx *ctx, r433b_batch const *b)
     dp.flip = b->sample_format == R433B_FMT_CS8 ? 0x80808080u : 0u;
     dp.enable_fm = ctx->enable_fm;
     dp.fpdm = (int)ctx->fpdm;
-    dp.lazy_fm = ctx->lazy_fm;
     dp.rate = b->samp_rate;
     dp.block_samples = block_bytes / SS;
     dp.lv = ctx->lv;
@@ -490,50 +564,12 @@ int r433b_process(r433b_ctx *ctx, r433b_batch const *b)
     };
 
     // slicer parameters: per device, scaled to this batch's sample rate on the host
-    std::vector<SlicerParams> sp(n_devs);
-    for (uint32_t i = 0; i < n_devs; ++i) {
-        sp[i] = scale_device(ctx->devs[i], b->samp_rate);
-        if (!ctx->gates.empty()) sp[i].gate = ctx->gates[i].min_bits;
-    }
-    // which devices look at OOK / FSK packages, in the order k_slice's warps take them
-    std::vector<unsigned> ook = slice_list(ctx->devs, 1), fsk = slice_list(ctx->devs, 2);
-    ctx->n_ook = (unsigned)ook.size();
-    ctx->n_fsk = (unsigned)fsk.size();
-    if (int r = dev_reserve(ctx, ctx->d_devparams, std::max<size_t>(1, n_devs) * sizeof(SlicerParams))) return r;
-    if (int r = dev_reserve(ctx, ctx->d_lists, (ook.size() + fsk.size() + 1) * sizeof(unsigned))) return r;
-    if (n_devs) CU(cudaMemcpy(ctx->d_devparams.p, sp.data(), n_devs * sizeof(SlicerParams), cudaMemcpyHostToDevice));
-    if (!ook.empty()) CU(cudaMemcpy(ctx->d_lists.p, ook.data(), ook.size() * sizeof(unsigned), cudaMemcpyHostToDevice));
-    if (!fsk.empty())
-        CU(cudaMemcpy((unsigned *)ctx->d_lists.p + ook.size(), fsk.data(), fsk.size() * sizeof(unsigned), cudaMemcpyHostToDevice));
+    if (int r = upload_slicer_tables(ctx, std::vector<uint32_t>{b->samp_rate}, st)) return r;
 
     if (ctx->pkg_cap < (size_t)b->n_streams * 16 + 1024) ctx->pkg_cap = (size_t)b->n_streams * 16 + 1024;
     if (ctx->pool_cap < ctx->pkg_cap * 128) ctx->pool_cap = ctx->pkg_cap * 128;
     if (ctx->arena_cap < total_bytes / 2 + (1u << 20)) ctx->arena_cap = total_bytes / 2 + (1u << 20);
 
-    unsigned stage_words = 0; // set below, before the first fill_slice() call
-    auto fill_slice = [&](SliceParams &q) {
-        q.pkgs = (r433b_package *)ctx->d_pkgs.p;
-        q.range = nullptr;
-        q.pulse_pool = (int const *)ctx->d_ppool.p;
-        q.gap_pool = (int const *)ctx->d_gpool.p;
-        q.dev = (SlicerParams const *)ctx->d_devparams.p;
-        q.n_devs = n_devs;
-        q.ook_list = (unsigned const *)ctx->d_lists.p;
-        q.fsk_list = (unsigned const *)ctx->d_lists.p + ook.size();
-        q.n_ook = ctx->n_ook;
-        q.n_fsk = ctx->n_fsk;
-        q.pairs = (r433b_pair *)ctx->d_pairs.p;
-        q.arena = (uint8_t *)ctx->d_arena.p;
-        q.arena_cap = ctx->arena_cap;
-        q.cursor = (unsigned long long *)ctx->d_cursor.p;
-        q.stage = (uint32_t *)ctx->d_stage.p;
-        q.stage_words = stage_words;
-    };
-    // k_slice always runs as a fixed grid whose CTAs fetch packages (GroupRange::next): every thread
-    // of that grid owns kStageWords of scratch for the staged single pass
-    unsigned const slice_grid = (unsigned)ctx->n_sms * kSliceCtasPerSm;
-    stage_words = ctx->stage_words;
-    if (int r = dev_reserve(ctx, ctx->d_stage, (size_t)slice_grid * kSliceThreads * stage_words * sizeof(uint32_t))) return r;
 
     // ---- pipelined path: host input cut into G TIME SLICES of every stream; the copy-in of slice
     //      k+1 and the copy-out of finished ranges overlap the kernels of slice k (three streams).
@@ -583,9 +619,6 @@ int r433b_process(r433b_ctx *ctx, r433b_batch const *b)
         dp.gap_pool = (int *)ctx->d_gpool.p;
         dp.pool_cap = (unsigned)std::min<size_t>(ctx->pool_cap, 0xffffffffu);
         dp.state = (StreamState *)ctx->d_state.p;
-        SliceParams q{};
-        fill_slice(q);
-        q.n_pkgs = dp.pkg_cap;
         GroupRange *d_rg = (GroupRange *)ctx->d_ranges.p;
         GroupRange *h_rg = (GroupRange *)ctx->h_ranges.p;
         unsigned const *d_cnt = (unsigned const *)ctx->d_counters.p;
@@ -620,9 +653,7 @@ int r433b_process(r433b_ctx *ctx, r433b_batch const *b)
             CU(cudaEventRecord(ctx->ev_det[g], ctx->s_det));
             R4_LAUNCH(k_mark, 1, 1, 0, ctx->s_det, d_rg + g, 2, d_cnt, d_cur);
             CU(cudaEventRecord(ctx->ev_t[4 * g + 2], ctx->s_det));
-            SliceParams qg = q;
-            qg.range = d_rg + g;
-            launch_slice(ctx, qg, slice_grid, ctx->s_det);
+            launch_slice(ctx, d_rg + g, dp.pkg_cap, 0, ctx->s_det);
             CU(cudaEventRecord(ctx->ev_t[4 * g + 3], ctx->s_det));
             R4_LAUNCH(k_mark, 1, 1, 0, ctx->s_det, d_rg + g, 3, d_cnt, d_cur);
             CU(cudaMemcpyAsync(h_rg + g, d_rg + g, sizeof(GroupRange), cudaMemcpyDeviceToHost, ctx->s_det));
@@ -748,42 +779,10 @@ int r433b_process(r433b_ctx *ctx, r433b_batch const *b)
         return fail(ctx, R433B_EOVERFLOW, "packages x devices exceeds the 32-bit pair index (r433b_package.first_pair)");
     ctx->n_pkgs = counters[0];
     ctx->pool_used = counters[1];
-    CU(cudaEventRecord(ctx->ev[2], st));
-
-    unsigned long long cursor[4] = {0, 0, 0, 0};
-    unsigned slice_launches = 0;
-    if (ctx->n_pkgs && n_devs) {
-        size_t pair_bytes = (size_t)ctx->n_pkgs * n_devs * sizeof(r433b_pair);
-        if (int r = dev_reserve(ctx, ctx->d_pairs, pair_bytes)) return r;
-        if (int r = dev_reserve(ctx, ctx->d_order, (size_t)ctx->n_pkgs * sizeof(unsigned))) return r;
-        if (int r = dev_reserve(ctx, ctx->d_ranges, sizeof(GroupRange))) return r;
-        for (int attempt = 0; attempt < 3; ++attempt) {
-            if (int r = dev_reserve(ctx, ctx->d_arena, ctx->arena_cap)) return r;
-            CU(cudaMemsetAsync(ctx->d_pairs.p, 0, pair_bytes, st));
-            CU(cudaMemsetAsync(ctx->d_cursor.p, 0, 64, st));
-            SliceParams q{};
-            fill_slice(q);
-            q.n_pkgs = ctx->n_pkgs;
-            GroupRange all{};
-            all.pkg_end = ctx->n_pkgs;
-            CU(cudaMemcpyAsync(ctx->d_ranges.p, &all, sizeof(all), cudaMemcpyHostToDevice, st));
-            q.range = (GroupRange *)ctx->d_ranges.p;
-            launch_slice(ctx, q, slice_grid, st);
-            CU(cudaGetLastError());
-            slice_launches++;
-            CU(cudaMemcpyAsync(cursor, ctx->d_cursor.p, sizeof(cursor), cudaMemcpyDeviceToHost, st));
-            CU(cudaStreamSynchronize(st));
-            if (!cursor[2]) break;
-            ctx->arena_cap = (size_t)cursor[0] + (1u << 20);
-            if (attempt == 2) return fail(ctx, R433B_EOVERFLOW, "event arena overflow");
-        }
-    }
-    ctx->event_bytes = cursor[0];
-    ctx->n_events = cursor[1];
-    ctx->n_gated = cursor[3];
+    GroupRange all{};
+    all.pkg_end = ctx->n_pkgs;
+    if (int r = slice_ranges(ctx, std::vector<GroupRange>{all}, ctx->n_pkgs, st)) return r;
     ctx->n_samples = used_bytes / SS;
-    CU(cudaEventRecord(ctx->ev[3], st));
-    CU(cudaEventSynchronize(ctx->ev[3]));
     cudaEventElapsedTime(&ctx->timing.h2d_ms, ctx->ev[0], ctx->ev[1]);
     ctx->timing.front_ms = 0;
     if (detect_launches) {
@@ -794,11 +793,9 @@ int r433b_process(r433b_ctx *ctx, r433b_batch const *b)
     ctx->timing.front_launches = detect_launches;
     ctx->timing.front_redone = counters[4];
     ctx->timing.front_repairs = counters[5];
-    cudaEventElapsedTime(&ctx->timing.slice_ms, ctx->ev[2], ctx->ev[3]);
     cudaEventElapsedTime(&ctx->timing.total_ms, ctx->ev[0], ctx->ev[3]);
     ctx->timing.d2h_ms = 0;
     ctx->timing.detect_launches = detect_launches;
-    ctx->timing.slice_launches = slice_launches;
     ctx->processed = true;
     return R433B_OK;
 }
@@ -1142,7 +1139,7 @@ int r433b_dispatch_r_devices_parallel(r433b_ctx *ctx, r433b_results const *res, 
 } // extern "C"
 
 // ------------------------------------------------ pulse-level I/O (SURVEY 8(f4)) -----------
-// Packages that never were IQ: `.ook` pulse files and RfRaw lines go straight to k_slice.
+// Packages that never were IQ: `.ook` pulse files and RfRaw lines go straight to the slicers.
 
 extern "C" {
 
@@ -1214,8 +1211,8 @@ void r433b_dump_logic_u8(uint8_t *buf, uint64_t len, uint64_t buf_offset, struct
 
 // run_ook_demods() / run_fsk_demods() on every package of the set (src/rtl_433.c:1755-1790, :1620-1650): the
 // slicers of all registered devices on the GPU, results fetched and replayed like those of r433b_process().
-// Packages may carry different sample rates (an RfRaw line is 1 MHz whatever the file's rate is): one k_slice
-// launch per distinct rate, each with the device widths scaled to that rate.
+// Packages may carry different sample rates (an RfRaw line is 1 MHz whatever the file's rate is): one package
+// range per distinct rate, sliced with the device widths scaled to that rate.
 int r433b_process_pulses(r433b_ctx *ctx, r433b_pulses const *ps)
 {
     if (!ctx || !ps) return fail(ctx, R433B_EINVAL, "null argument");
@@ -1243,8 +1240,8 @@ int r433b_process_pulses(r433b_ctx *ctx, r433b_pulses const *ps)
     std::vector<int32_t> pp, gp;
     pp.reserve(set.pulse.size());
     gp.reserve(set.gap.size());
-    struct RateRange { uint32_t rate, begin, end; };
-    std::vector<RateRange> rates;
+    std::vector<uint32_t> rates;
+    std::vector<GroupRange> ranges; // one per rate
     for (uint32_t j = 0; j < n; ++j) {
         PulseSet::Meta const &m = set.pk[order[j]];
         r433b_package &k = hp[j];
@@ -1261,20 +1258,21 @@ int r433b_process_pulses(r433b_ctx *ctx, r433b_pulses const *ps)
         k.first_pair = j * n_devs;
         pp.insert(pp.end(), set.pulse.begin() + m.first, set.pulse.begin() + m.first + m.count);
         gp.insert(gp.end(), set.gap.begin() + m.first, set.gap.begin() + m.first + m.count);
-        if (rates.empty() || rates.back().rate != m.rate) rates.push_back({m.rate, j, j});
-        rates.back().end = j + 1;
+        if (rates.empty() || rates.back() != m.rate) {
+            rates.push_back(m.rate);
+            ranges.push_back(GroupRange{});
+            ranges.back().pkg_begin = j;
+        }
+        ranges.back().pkg_end = j + 1;
     }
-    for (auto const &r : rates)
-        if (!r.rate) return fail(ctx, R433B_EINVAL, "a package has sample_rate 0");
+    for (uint32_t rate : rates)
+        if (!rate) return fail(ctx, R433B_EINVAL, "a package has sample_rate 0");
 
     ctx->n_pkgs = n;
     ctx->pool_used = (unsigned)pp.size();
     ctx->n_samples = 0;
     ctx->event_bytes = ctx->n_events = ctx->n_gated = 0;
     ctx->timing = r433b_timing{};
-    std::vector<unsigned> ook = slice_list(ctx->devs, 1), fsk = slice_list(ctx->devs, 2);
-    ctx->n_ook = (unsigned)ook.size();
-    ctx->n_fsk = (unsigned)fsk.size();
     if (n) { // the packages and their widths go to the device even without devices (r433b_analyze needs them)
         if (int r = dev_reserve(ctx, ctx->d_pkgs, (size_t)n * sizeof(r433b_package))) return r;
         if (int r = dev_reserve(ctx, ctx->d_ppool, pp.size() * sizeof(int) + 16)) return r;
@@ -1285,74 +1283,10 @@ int r433b_process_pulses(r433b_ctx *ctx, r433b_pulses const *ps)
         CU(cudaStreamSynchronize(st));
     }
     if (n && n_devs) {
-        size_t const pair_bytes = (size_t)n * n_devs * sizeof(r433b_pair);
-        if (int r = dev_reserve(ctx, ctx->d_pairs, pair_bytes)) return r;
-        if (int r = dev_reserve(ctx, ctx->d_ranges, rates.size() * sizeof(GroupRange))) return r;
-        if (int r = dev_reserve(ctx, ctx->d_order, (size_t)n * sizeof(unsigned))) return r;
-        if (int r = dev_reserve(ctx, ctx->d_devparams, rates.size() * n_devs * sizeof(SlicerParams))) return r;
-        if (int r = dev_reserve(ctx, ctx->d_lists, (ook.size() + fsk.size() + 1) * sizeof(unsigned))) return r;
-        if (int r = dev_reserve(ctx, ctx->d_cursor, 64)) return r;
-        unsigned const slice_grid = (unsigned)ctx->n_sms * kSliceCtasPerSm;
-        if (int r = dev_reserve(ctx, ctx->d_stage, (size_t)slice_grid * kSliceThreads * ctx->stage_words * sizeof(uint32_t))) return r;
         if (ctx->arena_cap < (size_t)(1u << 20)) ctx->arena_cap = 1u << 20;
-        std::vector<SlicerParams> sp(rates.size() * n_devs);
-        std::vector<GroupRange> rg(rates.size());
-        for (size_t g = 0; g < rates.size(); ++g) {
-            for (uint32_t i = 0; i < n_devs; ++i) {
-                sp[g * n_devs + i] = scale_device(ctx->devs[i], rates[g].rate);
-                if (!ctx->gates.empty()) sp[g * n_devs + i].gate = ctx->gates[i].min_bits;
-            }
-            rg[g] = GroupRange{};
-            rg[g].pkg_begin = rates[g].begin;
-            rg[g].pkg_end = rates[g].end;
-        }
-        CU(cudaMemcpyAsync(ctx->d_devparams.p, sp.data(), sp.size() * sizeof(SlicerParams), cudaMemcpyHostToDevice, st));
-        if (!ook.empty()) CU(cudaMemcpyAsync(ctx->d_lists.p, ook.data(), ook.size() * sizeof(unsigned), cudaMemcpyHostToDevice, st));
-        if (!fsk.empty())
-            CU(cudaMemcpyAsync((unsigned *)ctx->d_lists.p + ook.size(), fsk.data(), fsk.size() * sizeof(unsigned), cudaMemcpyHostToDevice, st));
-        unsigned long long cursor[4] = {0, 0, 0, 0};
-        CU(cudaEventRecord(ctx->ev[2], st));
-        for (int attempt = 0; attempt < 3; ++attempt) {
-            if (int r = dev_reserve(ctx, ctx->d_arena, ctx->arena_cap)) return r;
-            CU(cudaMemsetAsync(ctx->d_pairs.p, 0, pair_bytes, st));
-            CU(cudaMemsetAsync(ctx->d_cursor.p, 0, 64, st));
-            CU(cudaMemcpyAsync(ctx->d_ranges.p, rg.data(), rg.size() * sizeof(GroupRange), cudaMemcpyHostToDevice, st));
-            for (size_t g = 0; g < rates.size(); ++g) {
-                SliceParams q{};
-                q.pkgs = (r433b_package *)ctx->d_pkgs.p;
-                q.n_pkgs = n;
-                q.range = (GroupRange *)ctx->d_ranges.p + g;
-                q.pulse_pool = (int const *)ctx->d_ppool.p;
-                q.gap_pool = (int const *)ctx->d_gpool.p;
-                q.dev = (SlicerParams const *)ctx->d_devparams.p + g * n_devs;
-                q.n_devs = n_devs;
-                q.ook_list = (unsigned const *)ctx->d_lists.p;
-                q.fsk_list = (unsigned const *)ctx->d_lists.p + ook.size();
-                q.n_ook = ctx->n_ook;
-                q.n_fsk = ctx->n_fsk;
-                q.pairs = (r433b_pair *)ctx->d_pairs.p;
-                q.arena = (uint8_t *)ctx->d_arena.p;
-                q.arena_cap = ctx->arena_cap;
-                q.cursor = (unsigned long long *)ctx->d_cursor.p;
-                q.stage = (uint32_t *)ctx->d_stage.p;
-                q.stage_words = ctx->stage_words;
-                launch_slice(ctx, q, slice_grid, st);
-                CU(cudaGetLastError());
-                ctx->timing.slice_launches++;
-            }
-            CU(cudaMemcpyAsync(cursor, ctx->d_cursor.p, sizeof(cursor), cudaMemcpyDeviceToHost, st));
-            CU(cudaStreamSynchronize(st));
-            if (!cursor[2]) break;
-            ctx->arena_cap = (size_t)cursor[0] + (1u << 20);
-            if (attempt == 2) return fail(ctx, R433B_EOVERFLOW, "event arena overflow");
-        }
-        CU(cudaEventRecord(ctx->ev[3], st));
-        CU(cudaEventSynchronize(ctx->ev[3]));
-        cudaEventElapsedTime(&ctx->timing.slice_ms, ctx->ev[2], ctx->ev[3]);
+        if (int r = upload_slicer_tables(ctx, rates, st)) return r;
+        if (int r = slice_ranges(ctx, ranges, n, st)) return r;
         ctx->timing.total_ms = ctx->timing.slice_ms;
-        ctx->event_bytes = cursor[0];
-        ctx->n_events = cursor[1];
-        ctx->n_gated = cursor[3];
     }
     ctx->processed = true;
     return R433B_OK;

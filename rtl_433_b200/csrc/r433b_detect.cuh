@@ -142,7 +142,6 @@ struct DetectParams {
     int first_chunk;                   // start from reset_sdr_flow() state instead of the saved one
     struct StreamState *state;         // per-stream carried state between launches of one batch
     int use_mag, enable_fm, fpdm;
-    int lazy_fm;   // make FM windows on demand (needs the monotone FM filter: wrap_free)
     int want_stages; // the FM stage array is wanted for every sample (fm_out)
     unsigned flip; // XOR mask applied to every loaded word: 0x80808080 turns cs8 into cu8
     unsigned rate, block_samples;
@@ -1278,7 +1277,7 @@ __global__ void __launch_bounds__(kDetectWarps * 32, kDetectCtasPerSm) k_detect(
     int16_t *const am_stream = p.am + p.am_offsets[s];
     ChunkInfo const *const chunk_stream = p.chunks + p.am_offsets[s] / kChunk;
     // FM windows on demand need the rigorous state rebuild (monotone filter); the stage dump wants every sample
-    bool const lazy_fm = !fm_on || (p.wrap_free && p.lazy_fm && !p.want_stages);
+    bool const lazy_fm = !fm_on || (p.wrap_free && !p.want_stages);
     // the deferred carrier estimate re-makes FM for logged samples later: needs the state rebuild as well
     bool const defer_f1 = !fm_on || p.wrap_free != 0;
 

@@ -79,14 +79,12 @@ inline SlicerParams scale_device(r433b_device const &d, uint32_t rate)
 }
 
 
-// The device list k_slice walks for one package type (1 = OOK, 2 = FSK): indices into `devs` of the
-// devices run_ook_demods / run_fsk_demods hand such a package to (src/r_api.c:438-550), ordered so
-// that the 32 lanes of a warp walk the same code -- same slicer, then similar event cadence (reset
-// limit, short width; measured alternatives: event cadence first 61 ms, registration order 69 ms vs
-// 35 ms).  One k_slice work item is 32 consecutive slots: every LARGE modulation (>= 16 devices)
-// starts on a multiple of 32 (holes = kNoDevice) so that its warps run one slicer front end only;
-// the rare modulations share a warp (front ends one after the other, one shared back end) instead of
-// each costing a whole warp's pass over the pulses for a handful of lanes.
+// The device list k_slice2 walks for one package type (1 = OOK, 2 = FSK): each device
+// run_ook_demods / run_fsk_demods hand such a package to (src/r_api.c:438-550), once, as an index
+// into `devs`.  k_slice2's work items are device major, and the warps of the GPU fetch them in list
+// order, so the devices next to each other in the list are the ones that run side by side: sorted by
+// modulation, most warps of the GPU run the same slicer code at any moment (instruction cache); within
+// a modulation, reset limit and short width put devices of similar timing next to each other.
 inline std::vector<unsigned> slice_list(std::vector<r433b_device> const &devs, int package_type)
 {
     std::vector<unsigned> v;
@@ -99,17 +97,7 @@ inline std::vector<unsigned> slice_list(std::vector<r433b_device> const &devs, i
         if (x.short_width != y.short_width) return x.short_width < y.short_width;
         return a < c;
     });
-    std::vector<unsigned> out;
-    for (size_t i = 0; i < v.size(); ++i) {
-        if (i && devs[v[i]].modulation != devs[v[i - 1]].modulation) {
-            size_t n_same = 0;
-            for (size_t j = i; j < v.size() && devs[v[j]].modulation == devs[v[i]].modulation; ++j) n_same++;
-            if (n_same >= 16)
-                while (out.size() % 32) out.push_back(kNoDevice);
-        }
-        out.push_back(v[i]);
-    }
-    return out;
+    return v;
 }
 
 

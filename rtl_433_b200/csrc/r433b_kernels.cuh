@@ -2,8 +2,9 @@
 //
 //   k_detect (r433b_detect.cuh) : one WARP per capture stream, IQ -> packages.
 //   k_cf32_to_cs16              : float IQ captures to cs16 in front of k_detect.
-//   k_slice                     : one thread per (package, device): every pulse slicer on every package, events
-//                                 staged per thread and copied into the arena by the warp.
+//   k_bucket_count/scan/scatter : the packages of a range sorted by (type, length class) for k_slice2.
+//   k_slice2                    : one thread per (package, device), a warp = 32 packages of one device: every pulse
+//                                 slicer on every package, events staged per thread and copied into the arena by the warp.
 //   k_mark                      : one-thread bookkeeping between the launches of a pipelined batch.
 #pragma once
 #include <cuda_runtime.h>
@@ -42,7 +43,7 @@ __global__ void k_cf32_to_cs16(float4 const *in, uint2 *out, size_t n4)
     }
 }
 
-// ------------------------------------------------------------------------- k_slice -------
+// ------------------------------------------------------------------------- k_slice2 ------
 
 constexpr int kLenBuckets = 4; // length classes of packages: < 64, < 160, < 400 pulses, longer
 __host__ __device__ inline int len_bucket(unsigned num_pulses)
@@ -58,8 +59,8 @@ struct GroupRange {
     unsigned long long arena_begin, arena_end;
     unsigned long long events_end, gated_end;
     unsigned overflow;
-    unsigned next; // k_slice work counter: next (package, device group) item of this range, relative to pkg_begin
-    // k_bucket: the packages of the range sorted by (type, length class) in `order[pkg_begin + ...]` (k_slice2)
+    unsigned next; // k_slice2 work counter: next (device, package group) item of this range
+    // k_bucket: the packages of the range sorted by (type, length class) in `order[pkg_begin + ...]`
     unsigned seg_begin[2][kLenBuckets], seg_count[2][kLenBuckets], seg_fill[2][kLenBuckets];
     unsigned groups[2]; // per type: sum over the buckets of ceil(count / 32)
 };
@@ -85,155 +86,11 @@ __global__ void k_mark(GroupRange *r, int which, unsigned const *counters, unsig
     }
 }
 
-struct SliceParams {
-    r433b_package *pkgs;
-    unsigned n_pkgs;
-    GroupRange *range; // packages [pkg_begin, min(pkg_end, n_pkgs)) and the work counter
-    int const *pulse_pool, *gap_pool;
-    SlicerParams const *dev;  // per device, already scaled to the batch sample rate
-    unsigned n_devs;
-    unsigned const *ook_list, *fsk_list; // device indices taking OOK / FSK packages, grouped by modulation
-    unsigned n_ook, n_fsk;
-    r433b_pair *pairs;        // n_pkgs * n_devs, pre-zeroed
-    uint8_t *arena;
-    unsigned long long arena_cap;
-    unsigned long long *cursor; // [0] bytes reserved, [1] events stored, [2] overflow, [3] events dropped by a gate
-    uint32_t *stage;            // stage_words per thread of the (fixed, ranged) grid, or nullptr
-    unsigned stage_words;
-};
-
-constexpr int kSliceThreads = 128;
-constexpr unsigned kStageWords = 1024; // scratch words per k_slice thread (4 KiB): larger outputs take the second pass
-#ifndef R4_SLICE_CTAS
-#define R4_SLICE_CTAS 8
-#endif
-constexpr int kSliceCtasPerSm = R4_SLICE_CTAS; // 64 registers, 32 warps/SM.  k_slice2, gated, 4096 x 2^20 cu8: 6 CTAs/SM 7.0 ms, 8 -> 6.3, 12 -> 9.9
-                                               // (40 registers spill); the old k_slice liked 12 (12.6 ms vs 13.4 at 8)
-
-__global__ void __launch_bounds__(kSliceThreads, kSliceCtasPerSm) k_slice(SliceParams p)
-{
-    // A fixed grid of independent WARPS.  A work item is (package, group of 32 devices of the list
-    // that takes the package type); every warp fetches items from the range's counter until the
-    // range is exhausted.  (One CTA per package left most warps waiting at the CTA barrier for the
-    // slowest device group: 48 % of all stall samples.)
-    unsigned const lane = threadIdx.x & 31;
-    unsigned const groups = ((p.n_ook > p.n_fsk ? p.n_ook : p.n_fsk) + 31) / 32;
-    if (!groups) return;
-    unsigned const pk_begin = p.range->pkg_begin;
-    unsigned const pk_end = p.range->pkg_end < p.n_pkgs ? p.range->pkg_end : p.n_pkgs;
-    // Staging: the first run of the slicer writes its words into a per-thread scratch region; if
-    // every lane's output fitted, the warp reserves arena space and copies the regions over
-    // (coalesced, lane by lane) instead of running the slicers a second time.
-    uint32_t *stage = p.stage ? p.stage + ((size_t)blockIdx.x * kSliceThreads + threadIdx.x) * p.stage_words : nullptr;
-    unsigned const stage_words = stage ? p.stage_words : 0;
-    for (;;) {
-        unsigned item = 0;
-        if (lane == 0) item = atomicAdd(&p.range->next, 1u);
-        item = __shfl_sync(0xffffffffu, item, 0);
-        // device group major: at any moment most warps of the GPU run the same slicer (instruction cache)
-        if (pk_end <= pk_begin) break;
-        unsigned const n_rel = pk_end - pk_begin;
-        unsigned const g = item / n_rel, rel = item - g * n_rel;
-        if (g >= groups) break;
-        unsigned const pk = pk_begin + rel;
-        r433b_package const k = p.pkgs[pk];
-        unsigned const n_list = k.type == 1 ? p.n_ook : p.n_fsk;
-        unsigned const *list = k.type == 1 ? p.ook_list : p.fsk_list;
-        if (g == 0 && lane == 0) p.pkgs[pk].first_pair = pk * p.n_devs;
-        if (g * 32 >= n_list) continue;
-
-        PulseView pv;
-        pv.pulse = p.pulse_pool + k.pulse_off;
-        pv.gap = p.gap_pool + k.pulse_off;
-        pv.n = k.num_pulses;
-
-        unsigned const slot = g * 32 + lane;
-        unsigned const dev = slot < n_list ? list[slot] : kNoDevice;
-        bool const active = dev != kNoDevice;
-        unsigned bytes = 0, nev = 0, ng1 = 0, ngN = 0;
-        unsigned long long off = 0;
-        bool fits = false;
-        SlicerParams sp;
-        if (active) sp = p.dev[dev];
-        // pass 0 counts (and stages), pass 1 stores; one copy of the slicer code serves both
-#pragma unroll 1
-        for (int pass = 0; pass < 2; ++pass) {
-            if (pass == 1) {
-                // warp-aggregated reservation in the event arena
-                unsigned incl = bytes;
-#pragma unroll
-                for (int o = 1; o < 32; o <<= 1) {
-                    unsigned v = __shfl_up_sync(0xffffffffu, incl, o);
-                    if ((int)lane >= o) incl += v;
-                }
-                unsigned total = __shfl_sync(0xffffffffu, incl, 31);
-                unsigned evs = nev, dropped = ng1 + ngN;
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) {
-                    evs += __shfl_xor_sync(0xffffffffu, evs, o);
-                    dropped += __shfl_xor_sync(0xffffffffu, dropped, o);
-                }
-                unsigned long long wbase = 0;
-                if (lane == 0 && total) {
-                    wbase = atomicAdd(p.cursor, (unsigned long long)total);
-                    atomicAdd(p.cursor + 1, (unsigned long long)evs);
-                }
-                if (lane == 0 && dropped) atomicAdd(p.cursor + 3, (unsigned long long)dropped);
-                wbase = __shfl_sync(0xffffffffu, wbase, 0);
-                off = wbase + incl - bytes;
-                fits = off + bytes <= p.arena_cap;
-                if (active && bytes && !fits) atomicOr(p.cursor + 2, 1ull);
-                bool const staged = bytes <= stage_words * 4;
-                if (__all_sync(0xffffffffu, !active || !bytes || staged)) {
-                    __syncwarp();
-                    unsigned todo = __ballot_sync(0xffffffffu, active && bytes && fits);
-                    while (todo) {
-                        int const l = __ffs(todo) - 1;
-                        todo &= todo - 1;
-                        unsigned const wl = __shfl_sync(0xffffffffu, bytes, l) / 4;
-                        unsigned long long const ol = __shfl_sync(0xffffffffu, off, l);
-                        uint32_t const *from = stage + ((long long)l - (long long)lane) * (long long)stage_words;
-                        uint32_t *to = reinterpret_cast<uint32_t *>(p.arena + ol);
-                        for (unsigned i = lane; i < wl; i += 32) __stcs(to + i, from[i]);
-                    }
-                    __syncwarp();
-                    break;
-                }
-            }
-            if (active && (pass == 0 || (bytes && fits))) {
-                EventWriter w;
-                if (pass)
-                    w.init(reinterpret_cast<uint32_t *>(p.arena + off), bytes / 4, (unsigned)sp.gate);
-                else
-                    w.init(stage, stage_words, (unsigned)sp.gate);
-                slice_dispatch(pv, sp, w);
-                if (pass == 0) {
-                    bytes = w.committed * 4;
-                    nev = w.events;
-                    ng1 = w.gated1;
-                    ngN = w.gatedN;
-                }
-            }
-        }
-        if (active) {
-            r433b_pair pr;
-            pr.offset = off;
-            pr.bytes = bytes;
-            pr.events = nev;
-            pr.gated_single = ng1;
-            pr.gated_multi = ngN;
-            p.pairs[(size_t)pk * p.n_devs + dev] = pr;
-        }
-    }
-}
-
-// ------------------------------------------------------------------------- k_slice2 ------
-//
-// The same slicers with the work turned by ninety degrees: the 32 lanes of a warp are 32 PACKAGES looked at by ONE
-// device.  Lanes of k_slice (32 devices on one package) interpret the same pulse with 32 different sets of limits
-// and so want 32 different things from the bit writer; here all lanes carry the same limits, walk packages of the
-// same type and similar length (k_bucket), and pulse n of one burst is the same kind of thing as pulse n of another
-// -- the lanes differ in data (which bit), far less in control flow.
+// The 32 lanes of a k_slice2 warp are 32 PACKAGES looked at by ONE device.  Lanes that were 32 devices on one
+// package would interpret the same pulse with 32 different sets of limits and so want 32 different things from the
+// bit writer; here all lanes carry the same limits, walk packages of the same type and similar length (k_bucket), and
+// pulse n of one burst is the same kind of thing as pulse n of another -- the lanes differ in data (which bit), far
+// less in control flow.
 
 // Sort the packages of a range by (type, length class) into order[pkg_begin ...): count, scan, scatter -- three small
 // launches without a block barrier (grid-stride loops; the range is only known on the device).  The count pass also
@@ -276,14 +133,31 @@ __global__ void __launch_bounds__(kBucketThreads) k_bucket_scatter(GroupRange *r
     }
 }
 
-struct Slice2Params {
-    SliceParams s;
+struct SliceParams {
+    r433b_package const *pkgs;
+    GroupRange *range; // the packages of the range (k_bucket's segments) and the work counter
     unsigned const *order; // k_bucket's output
+    int const *pulse_pool, *gap_pool;
+    SlicerParams const *dev;  // per device, already scaled to the sample rate of the range
+    unsigned n_devs;
+    unsigned const *ook_list, *fsk_list; // device indices taking OOK / FSK packages, grouped by modulation
+    unsigned n_ook, n_fsk;
+    r433b_pair *pairs;        // n_pkgs * n_devs, pre-zeroed
+    uint8_t *arena;
+    unsigned long long arena_cap;
+    unsigned long long *cursor; // [0] bytes reserved, [1] events stored, [2] overflow, [3] events dropped by a gate
+    uint32_t *stage;            // stage_words per thread of the (fixed) grid
+    unsigned stage_words;       // always kStageWords, passed at run time: with the compile-time constant the compiler
+                                // allocates k_slice2's registers differently and it ran 0.7 % slower (H100 80GB HBM3, 400 W)
 };
 
-__global__ void __launch_bounds__(kSliceThreads, kSliceCtasPerSm) k_slice2(Slice2Params q)
+constexpr int kSliceThreads = 128;
+constexpr unsigned kStageWords = 1024; // scratch words per k_slice2 thread (4 KiB): larger outputs take the second pass
+constexpr int kSliceCtasPerSm = 8; // 64 registers, 32 warps/SM.  Gated, 4096 x 2^20 cu8: 6 CTAs/SM 7.0 ms, 8 -> 6.3,
+                                   // 12 -> 9.9 (40 registers spill)
+
+__global__ void __launch_bounds__(kSliceThreads, kSliceCtasPerSm) k_slice2(SliceParams p)
 {
-    SliceParams const &p = q.s;
     unsigned const lane = threadIdx.x & 31;
     GroupRange const *rg = p.range;
     unsigned const pk_begin = rg->pkg_begin;
@@ -304,7 +178,6 @@ __global__ void __launch_bounds__(kSliceThreads, kSliceCtasPerSm) k_slice2(Slice
         unsigned const slot = rel / groups;
         unsigned g = rel - slot * groups;
         unsigned const dev = (t ? p.fsk_list : p.ook_list)[slot];
-        if (dev == kNoDevice) continue; // alignment hole of the device list (k_slice's layout)
         int b = 0;
         for (; b < kLenBuckets - 1; ++b) {
             unsigned const gb = (rg->seg_count[t][b] + 31) / 32;
@@ -313,7 +186,7 @@ __global__ void __launch_bounds__(kSliceThreads, kSliceCtasPerSm) k_slice2(Slice
         }
         unsigned const in_seg = g * 32 + lane;
         bool const active = in_seg < rg->seg_count[t][b];
-        unsigned const pk = active ? q.order[pk_begin + rg->seg_begin[t][b] + in_seg] : 0;
+        unsigned const pk = active ? p.order[pk_begin + rg->seg_begin[t][b] + in_seg] : 0;
         SlicerParams const sp = p.dev[dev];
         PulseView pv;
         pv.pulse = p.pulse_pool;

@@ -7,7 +7,7 @@
 //             VCD                         pulse_data_print_vcd()     src/pulse_data.c:102-121
 //             logic.u8                    pulse_data_dump_raw()      src/pulse_data.c:58-68
 //
-// A loaded set of packages goes to the GPU through r433b_process_pulses() (k_slice only): the same slicers,
+// A loaded set of packages goes to the GPU through r433b_process_pulses() (the slicer stage only): the same slicers,
 // the same event arena, the same replay as packages that came out of k_detect.  Host-only, no CUDA here.
 #pragma once
 #include <cstdarg>

@@ -47,8 +47,6 @@ R4_HD double dmul(double a, double b) { volatile double r = a * b; return r; }
 
 // Integer timing of one device at one sample rate.  Derived ON THE HOST (r433b_host.cpp) with
 // the reference's float expressions (src/pulse_slicer.c:70-91) and shipped as integers.
-constexpr unsigned kNoDevice = 0xffffffffu; // hole in a k_slice device list (alignment padding)
-
 struct SlicerParams {
     int modulation;
     int ok; // bit 0: all six scaled widths survived (the check of every slicer but RZI, src/pulse_slicer.c:79-84);

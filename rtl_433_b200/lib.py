@@ -380,7 +380,7 @@ class Context:
         self._check(self.L.r433b_process(self.h, C.byref(b)))
 
     def process_pulses(self, pulses):
-        """All slicers on every package of a Pulses set (k_slice only); then fetch()/dispatch as usual."""
+        """All slicers on every package of a Pulses set (the slicer stage only); then fetch()/dispatch as usual."""
         self._keep = pulses
         self._check(self.L.r433b_process_pulses(self.h, pulses.h))
 

@@ -354,7 +354,7 @@ int16_t const *hc_am(void *p) { return ((Hc *)p)->am.data(); }
 int16_t const *hc_fm(void *p) { return ((Hc *)p)->fm.data(); }
 
 
-// the device list k_slice walks for one package type (rtl_433_b200/csrc/r433b_host.hpp: slice_list)
+// the device list k_slice2 walks for one package type (rtl_433_b200/csrc/r433b_host.hpp: slice_list)
 int hc_slice_list(void *p, int package_type, uint32_t *out, int cap)
 {
     std::vector<unsigned> v = slice_list(((Hc *)p)->devs, package_type);

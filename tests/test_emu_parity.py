@@ -1,4 +1,4 @@
-"""CPU: the kernels' own source (k_detect, k_slice, k_cf32_to_cs16 and the C ABI around them) executed by
+"""CPU: the kernels' own source (k_detect, k_slice2, k_cf32_to_cs16 and the C ABI around them) executed by
 the SIMT emulator (tests/emu.py, tests/simt/) under the SAME parity tests the GPU suite runs on the H100:
 every test function below is imported from the `-m gpu` modules and compares, through the C ABI, with the
 oracle (and the compiled reference).  Two lane schedules (ascending here, descending in
@@ -38,9 +38,9 @@ import test_pulse_io  # noqa: E402
 
 
 @test_pulse_io.needs_ref
-def test_emu_loaded_packages_through_k_slice():
+def test_emu_loaded_packages_through_k_slice2():
     """r433b_process_pulses (SURVEY 8(f4)) under the emulator: the body of the -m gpu test."""
-    test_pulse_io.loaded_packages_through_k_slice()
+    test_pulse_io.loaded_packages_through_k_slice2()
 
 
 def test_emu_reverse_schedule(devices):
@@ -66,7 +66,7 @@ import test_gates  # noqa: E402
 
 
 def test_emu_gated_run_is_the_filtered_ungated_run():
-    """Decoder length gates in k_slice (SURVEY 8(f1)) under the emulator: the body of the -m gpu test."""
+    """Decoder length gates in k_slice2 (SURVEY 8(f1)) under the emulator: the body of the -m gpu test."""
     test_gates.gated_run_is_the_filtered_ungated_run()
 
 
@@ -86,28 +86,6 @@ def test_emu_analyzer_matches_the_reference():
 
 def test_emu_submit_wait_ping_pong():
     test_gates.submit_wait_ping_pong()
-
-
-def test_emu_slice_v1_still_exact(devices):
-    """R433B_SLICE_V1=1 keeps the round-1 formulation of the slicer kernel (lanes = devices on one package) for A/B
-    timing; it has to stay exact too."""
-    import subprocess
-    import sys
-    code = ("import os,sys;sys.path.insert(0,%r);sys.path.insert(0,%r);import emu;emu.use();import numpy as np;"
-            "import helpers;from oracle import orc;from rtl_433_b200 import lib,synth;"
-            "devs=lib.default_device_table();c=lib.Context(0);c.set_devices(devs);c.set_gates(lib.default_gates(devs));"
-            "o=orc.Oracle(store_bitbuffers=False);o.add_devices(devs);"
-            "x=synth.ook_stream(3,n_samples=1<<18,n_bursts=2);"
-            "c.process(x,np.array([0,x.nbytes],np.uint64),2,250000,433920000);r=c.fetch();"
-            "g=helpers.gpu_stream_results(c,0);w=o.run(x,2);gates=lib.default_gates(devs);"
-            "keep=[(e['package'],e['dev'],e['hash']) for e in g['events']];"
-            "c.set_gates(None);c.process(x,np.array([0,x.nbytes],np.uint64),2,250000,433920000);c.fetch();"
-            "full=helpers.gpu_stream_results(c,0);"
-            "bad=len(helpers.compare_results(w,full,'v1',stages=False));"
-            "want=[(e['package'],e['dev'],e['hash']) for e in full['events'] if not (e['num_rows']>=1 and e['max_bits']<gates[e['dev']][0])];"
-            "sys.exit(1 if bad or keep!=want or not keep else 0)") % (os.path.dirname(os.path.abspath(__file__)), emu.ROOT)
-    env = dict(os.environ, R433B_SLICE_V1="1")
-    assert subprocess.call([sys.executable, "-c", code], env=env) == 0
 
 
 @test_analyzer.needs_ref

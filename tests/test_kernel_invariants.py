@@ -36,10 +36,10 @@ def test_fm_filter_state_rebuild_is_sound_and_usually_converges():
     assert L.hc_check_bracket_rebuild(9, 200, 0, 250000, 1024, 0) < 200
 
 
-def test_slice_work_lists_cover_every_device_once_and_align_large_modulations():
-    """k_slice's work items are 32 consecutive slots of these lists: every device that takes the
-    package type appears exactly once, holes are padding only, a modulation with >= 16 devices
-    starts on a warp boundary, and devices of one modulation stay together."""
+def test_slice_work_lists_cover_every_device_once_in_slicer_order():
+    """k_slice2 takes these lists device by device: every device that takes the package type appears
+    exactly once and nothing else does; devices of one modulation stay together, modulations ascend,
+    and within a modulation the order is (reset_limit, short_width), then registration."""
     devs = lib.default_device_table(include_disabled=True)
     hc = helpers.HostCore()
     hc.add_devices(devs)
@@ -47,20 +47,9 @@ def test_slice_work_lists_cover_every_device_once_and_align_large_modulations():
     for ptype, takes in ((1, lambda m: 3 <= m <= 13 and m != 7), (2, lambda m: 16 <= m <= 18)):
         buf = np.zeros(4096, np.uint32)
         n = hc.L.hc_slice_list(hc.h, ptype, buf.ctypes.data, len(buf))
-        lst = buf[:n]
-        real = [int(x) for x in lst if x != 0xFFFFFFFF]
+        lst = [int(x) for x in buf[:n]]
         want = [i for i, d in enumerate(devs) if takes(d["modulation"])]
-        assert sorted(real) == want
-        mods = [devs[i]["modulation"] for i in real]
-        assert mods == sorted(mods), "devices of one modulation are contiguous, modulations ascending"
-        count = {m: mods.count(m) for m in set(mods)}
-        seen = set()
-        for slot, x in enumerate(lst):
-            if x == 0xFFFFFFFF:
-                continue
-            m = devs[int(x)]["modulation"]
-            if m not in seen:
-                seen.add(m)
-                if count[m] >= 16:
-                    assert slot % 32 == 0, f"modulation {m} ({count[m]} devices) starts at slot {slot}"
-        assert n - len(real) < 32 * len(count)
+        assert sorted(lst) == want
+        # the device table holds floats (r433b_device): compare in float32 as slice_list does
+        key = [(devs[i]["modulation"], np.float32(devs[i]["reset_limit"]), np.float32(devs[i]["short_width"]), i) for i in lst]
+        assert key == sorted(key), "modulations contiguous and ascending, then (reset_limit, short_width)"

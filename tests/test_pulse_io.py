@@ -2,7 +2,7 @@
 (host functions of libr433b.so, rtl_433_b200/csrc/r433b_pulses.hpp) against the compiled reference
 (pulse_data_load, rfraw_parse, pulse_data_dump, pulse_data_print_vcd, pulse_data_dump_raw of oracle/_ref) and
 against the committed golden fixture (tests/golden/pulse_io.json, generated from the reference by
-tools/make_golden.py).  The -m gpu part sends loaded packages through k_slice and compares every bitbuffer
+tools/make_golden.py).  The -m gpu part sends loaded packages through k_slice2 and compares every bitbuffer
 with run_ook_demods() / run_fsk_demods() of the reference on the same pulse_data_t."""
 import json
 import os
@@ -245,12 +245,12 @@ def sliced_by_reference(ref, pd):
 
 @pytest.mark.gpu
 @needs_ref
-def test_loaded_packages_through_k_slice():
+def test_loaded_packages_through_k_slice2():
     """`.ook` text and RfRaw lines -> r433b_process_pulses -> every bitbuffer equal to the reference's slicers."""
-    loaded_packages_through_k_slice()
+    loaded_packages_through_k_slice2()
 
 
-def loaded_packages_through_k_slice():
+def loaded_packages_through_k_slice2():
     devices = lib.default_device_table()
     ctx = lib.Context(0)
     ctx.set_devices(devices)
@@ -299,14 +299,25 @@ def loaded_packages_through_k_slice():
         fsk_pd["gap"][n - 1] = 30000
         ps.add(fsk_pd, stream=3)
         ps.add(random_pulse_data(rng), stream=3)
+        # long pulses through the PCM devices: the row spill (src/bitbuffer.c:39-54) fills the whole 50 x 128 bytes
+        # of the bitbuffer, so one device's events for this package outgrow the 4 KiB a k_slice2 thread stages them in
+        long_pd = np.zeros(1, lib.PULSE_DATA_DTYPE)[0]
+        long_pd["sample_rate"] = 250000
+        long_pd["num_pulses"] = 40
+        long_pd["pulse"][:40] = 20000
+        long_pd["gap"][:40] = 100
+        long_pd["gap"][39] = 250000
+        ps.add(long_pd, stream=3)
 
         want_sets = [list(refh.load_ook(texts[0], 250000)), list(refh.load_ook(texts[1], 250000)),
-                     list(refh.load_ook(mixed, 1024000)), [refh.rfraw(cases["rfraw_b1_line"].strip()), fsk_pd, ps.get(len(ps) - 1)]]
+                     list(refh.load_ook(mixed, 1024000)),
+                     [refh.rfraw(cases["rfraw_b1_line"].strip()), fsk_pd, ps.get(len(ps) - 2), long_pd]]
         assert sum(len(w) for w in want_sets) == len(ps)
         assert len({int(p["sample_rate"]) for w in want_sets for p in w}) >= 3
 
         ctx.process_pulses(ps)
-        ctx.fetch()
+        res = ctx.fetch()
+        assert (res["pairs"]["bytes"] > 4096).any(), "no device's events outgrew the staging region"
         total_events = 0
         for s, want in enumerate(want_sets):
             got = helpers.gpu_stream_results(ctx, s)

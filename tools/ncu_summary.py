@@ -46,7 +46,7 @@ rd, wr, dur = num("dram__bytes_read.sum"), num("dram__bytes_write.sum"), num("gp
 lines += ["", f"DRAM traffic per launch: {rd / 1e9:.3f} GB read + {wr / 1e9:.3f} GB written = {(rd + wr) / 1e9:.3f} GB in {dur * 1e3:.2f} ms "
           f"(under the profiler) = {(rd + wr) / dur / 1e9:.1f} GB/s"]
 if traffic_json:
-    short = "k_front" if "k_front" in kernel else "k_detect" if "k_detect" in kernel else "k_slice2" if "k_slice2" in kernel else "k_slice" if "k_slice" in kernel else kernel
+    short = "k_front" if "k_front" in kernel else "k_detect" if "k_detect" in kernel else "k_slice2" if "k_slice2" in kernel else kernel
     wl = os.environ.get("NCU_WORKLOAD", "ook_cu8_250k")
     try:
         allt = json.load(open(traffic_json))
@@ -99,7 +99,7 @@ for (fn, ln), (sm, ins, text) in sorted(agg.items(), key=lambda kv: -kv[1][0])[:
 if "k_detect" in kernel:
     fn = subprocess.run([sys.executable, os.path.join(ROOT, "tools", "ncu_funcs.py"), rep, "k_detectILi2"], capture_output=True, text=True).stdout
     lines += ["", "## by device function (tools/ncu_funcs.py; the phases of the walk are separate functions)", "", fn.rstrip()]
-kind = "slice" if "k_slice" in kernel else None
+kind = "slice" if "k_slice2" in kernel else None
 if kind:
     reg = subprocess.run([sys.executable, os.path.join(ROOT, "tools", "ncu_regions.py"), rep, kind], capture_output=True, text=True).stdout
     lines += ["", "## by code region (tools/ncu_regions.py; IQ samples of the 4096 x 2^20 workload)", "", reg.rstrip()]

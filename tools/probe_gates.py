@@ -2,7 +2,7 @@
 """Derive the decoder length gates (SURVEY 8(f1)) from the UNMODIFIED reference decoders (oracle/_ref) and write
 rtl_433_b200/data/gates_25.12.json: for every protocol the largest T <= MAX_BITS such that every probed event whose
 rows all hold fewer than T bits is rejected by decode_fn with one constant code c <= 0 and no output (exhaustive over
-single rows, sampled over multi-row buffers: oracle/ref_harness.c:refh_probe_gate).  An r433b_gate {T, c} lets k_slice
+single rows, sampled over multi-row buffers: oracle/ref_harness.c:refh_probe_gate).  An r433b_gate {T, c} lets k_slice2
 drop such events on the device and only count them (one-row and several-row events separately: many decoders test
 num_rows first); the host adds the counts to decode_events / decode_fails[-code], so
 the decoders' statistics stay what account_event() (src/pulse_slicer.c:26-66) would have produced.  Run in the build
