@@ -192,6 +192,10 @@ int r433b_create(int cuda_device, r433b_ctx **out)
     cudaFuncSetAttribute((void const *)k_front<4>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     cudaFuncSetAttribute((void const *)k_detect<2>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     cudaFuncSetAttribute((void const *)k_detect<4>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    // k_slice2: the carve-out that holds kSliceCtasPerSm CTAs of windows (plus the 1 KiB the system reserves per CTA)
+    // out of H100's 228 KiB per SM; the rest stays L1 for the pulse loads
+    cudaFuncSetAttribute((void const *)k_slice2, cudaFuncAttributePreferredSharedMemoryCarveout,
+                         (int)((kSliceCtasPerSm * (sizeof(g_slice_win) + sizeof(g_slice_seg) + 1024) * 100 + 228 * 1024 - 1) / (228 * 1024)));
     for (auto &v : ctx->ev) cudaEventCreate(&v);
     cudaStreamCreateWithFlags(&ctx->s_in, cudaStreamNonBlocking);
     cudaStreamCreateWithFlags(&ctx->s_det, cudaStreamNonBlocking);
@@ -356,7 +360,6 @@ void launch_slice(r433b_ctx *ctx, GroupRange *range, unsigned n_pkgs, unsigned r
     q.arena_cap = ctx->arena_cap;
     q.cursor = (unsigned long long *)ctx->d_cursor.p;
     q.stage = (uint32_t *)ctx->d_stage.p;
-    q.stage_words = kStageWords;
     unsigned const bgrid = (unsigned)ctx->n_sms * 2;
     R4_LAUNCH(k_bucket_count, bgrid, kBucketThreads, 0, st, range, pkgs, n_pkgs, n_devs);
     R4_LAUNCH(k_bucket_scan, 1, 1, 0, st, range);

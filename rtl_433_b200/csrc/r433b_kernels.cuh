@@ -146,9 +146,7 @@ struct SliceParams {
     uint8_t *arena;
     unsigned long long arena_cap;
     unsigned long long *cursor; // [0] bytes reserved, [1] events stored, [2] overflow, [3] events dropped by a gate
-    uint32_t *stage;            // stage_words per thread of the (fixed) grid
-    unsigned stage_words;       // always kStageWords, passed at run time: with the compile-time constant the compiler
-                                // allocates k_slice2's registers differently and it ran 0.7 % slower (H100 80GB HBM3, 400 W)
+    uint32_t *stage;            // kStageWords per thread of the (fixed) grid
 };
 
 constexpr int kSliceThreads = 128;
@@ -156,17 +154,28 @@ constexpr unsigned kStageWords = 1024; // scratch words per k_slice2 thread (4 K
 constexpr int kSliceCtasPerSm = 8; // 64 registers, 32 warps/SM.  Gated, 4096 x 2^20 cu8: 6 CTAs/SM 7.0 ms, 8 -> 6.3,
                                    // 12 -> 9.9 (40 registers spill)
 
+// k_slice2's shared memory: the threads' write-combining windows, a column each (a lane always hits its own bank),
+// and per thread the first word of its output in the warp's arena range and the first one still in its window
+__shared__ uint32_t g_slice_win[kSliceWindow][kSliceThreads];
+__shared__ unsigned g_slice_seg[2][kSliceThreads];
+struct SliceWindow {
+    static constexpr bool kOn = true;
+    __device__ __forceinline__ static uint32_t &slot(unsigned s) { return g_slice_win[s][threadIdx.x]; }
+};
+
+// One slicing pass per (package, device) item: the events go through the thread's window into its scratch, and the
+// warp copies the outputs of its 32 lanes, which are one contiguous arena range, in whole lines.  A warp with a lane
+// whose output outgrows the scratch slices again, straight into the arena.
 __global__ void __launch_bounds__(kSliceThreads, kSliceCtasPerSm) k_slice2(SliceParams p)
 {
-    unsigned const lane = threadIdx.x & 31;
+    unsigned const lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     GroupRange const *rg = p.range;
     unsigned const pk_begin = rg->pkg_begin;
     unsigned const groups_ook = rg->groups[0], groups_fsk = rg->groups[1];
     // items: device major (at any moment most warps of the GPU run the same device, so the same code), OOK devices
     // on the OOK packages first
     unsigned const items_ook = p.n_ook * groups_ook, items = items_ook + p.n_fsk * groups_fsk;
-    uint32_t *stage = p.stage ? p.stage + ((size_t)blockIdx.x * kSliceThreads + threadIdx.x) * p.stage_words : nullptr;
-    unsigned const stage_words = stage ? p.stage_words : 0;
+    uint32_t *stage = p.stage + ((size_t)blockIdx.x * kSliceThreads + threadIdx.x) * kStageWords;
     for (;;) {
         unsigned item = 0;
         if (lane == 0) item = atomicAdd(&p.range->next, 1u);
@@ -198,74 +207,70 @@ __global__ void __launch_bounds__(kSliceThreads, kSliceCtasPerSm) k_slice2(Slice
             pv.gap = p.gap_pool + k.pulse_off;
             pv.n = k.num_pulses;
         }
-        unsigned bytes = 0, nev = 0, ng1 = 0, ngN = 0;
-        unsigned long long off = 0;
-        bool fits = false;
-#pragma unroll 1
-        for (int pass = 0; pass < 2; ++pass) {
-            if (pass == 1) {
-                unsigned incl = bytes;
+        unsigned bytes = 0, nev = 0, ng1 = 0, ngN = 0, wb = 0;
+        if (active) {
+            EventWriterT<SliceWindow> w;
+            w.init(stage, kStageWords, (unsigned)sp.gate);
+            slice_dispatch(pv, sp, w);
+            bytes = w.committed * 4;
+            wb = w.wb;
+            nev = w.events;
+            ng1 = w.gated1;
+            ngN = w.gatedN;
+        }
+        unsigned incl = bytes;
 #pragma unroll
-                for (int o = 1; o < 32; o <<= 1) {
-                    unsigned v = __shfl_up_sync(0xffffffffu, incl, o);
-                    if ((int)lane >= o) incl += v;
-                }
-                unsigned total = __shfl_sync(0xffffffffu, incl, 31);
-                unsigned evs = nev, dropped = ng1 + ngN;
+        for (int o = 1; o < 32; o <<= 1) {
+            unsigned v = __shfl_up_sync(0xffffffffu, incl, o);
+            if ((int)lane >= o) incl += v;
+        }
+        unsigned const total = __shfl_sync(0xffffffffu, incl, 31);
+        unsigned evs = nev, dropped = ng1 + ngN;
 #pragma unroll
-                for (int o = 16; o > 0; o >>= 1) {
-                    evs += __shfl_xor_sync(0xffffffffu, evs, o);
-                    dropped += __shfl_xor_sync(0xffffffffu, dropped, o);
-                }
-                unsigned long long wbase = 0;
-                if (lane == 0 && total) {
-                    wbase = atomicAdd(p.cursor, (unsigned long long)total);
-                    atomicAdd(p.cursor + 1, (unsigned long long)evs);
-                }
-                if (lane == 0 && dropped) atomicAdd(p.cursor + 3, (unsigned long long)dropped);
-                wbase = __shfl_sync(0xffffffffu, wbase, 0);
-                off = wbase + incl - bytes;
-                fits = off + bytes <= p.arena_cap;
-                if (active && bytes && !fits) atomicOr(p.cursor + 2, 1ull);
-                bool const staged = bytes <= stage_words * 4;
-                if (__all_sync(0xffffffffu, !active || !bytes || staged)) {
-                    __syncwarp();
-                    // short outputs (the usual case: a few events of a few words) are copied by their own lane -- the
-                    // lanes' arena regions lie back to back, so neighbouring lanes hit the same lines; only long ones
-                    // are worth a coalesced copy by the whole warp
-                    unsigned const my_words = active && fits ? bytes / 4 : 0;
-                    if (my_words <= 16) {
-                        uint32_t *to = reinterpret_cast<uint32_t *>(p.arena + off);
-                        for (unsigned i = 0; i < my_words; ++i) __stcs(to + i, stage[i]);
-                    }
-                    unsigned todo = __ballot_sync(0xffffffffu, my_words > 16);
-                    while (todo) {
-                        int const l = __ffs(todo) - 1;
-                        todo &= todo - 1;
-                        unsigned const wl = __shfl_sync(0xffffffffu, bytes, l) / 4;
-                        unsigned long long const ol = __shfl_sync(0xffffffffu, off, l);
-                        uint32_t const *from = stage + ((long long)l - (long long)lane) * (long long)stage_words;
-                        uint32_t *to = reinterpret_cast<uint32_t *>(p.arena + ol);
-                        for (unsigned i = lane; i < wl; i += 32) __stcs(to + i, from[i]);
-                    }
-                    __syncwarp();
-                    break;
-                }
+        for (int o = 16; o > 0; o >>= 1) {
+            evs += __shfl_xor_sync(0xffffffffu, evs, o);
+            dropped += __shfl_xor_sync(0xffffffffu, dropped, o);
+        }
+        unsigned long long wbase = 0;
+        if (lane == 0 && total) {
+            wbase = atomicAdd(p.cursor, (unsigned long long)total);
+            atomicAdd(p.cursor + 1, (unsigned long long)evs);
+        }
+        if (lane == 0 && dropped) atomicAdd(p.cursor + 3, (unsigned long long)dropped);
+        wbase = __shfl_sync(0xffffffffu, wbase, 0);
+        unsigned long long const off = wbase + incl - bytes;
+        bool const fits = off + bytes <= p.arena_cap;
+        if (active && bytes && !fits) atomicOr(p.cursor + 2, 1ull);
+        if (__all_sync(0xffffffffu, bytes <= kStageWords * 4)) {
+            // word i of the warp's range [wbase, wbase + total) belongs to the last lane whose output starts at or
+            // before i; the lanes take 32 consecutive words, aligned to a 128-byte line, at a time
+            unsigned const first = (incl - bytes) / 4;
+            g_slice_seg[0][threadIdx.x] = first;
+            g_slice_seg[1][threadIdx.x] = first + wb;
+            __syncwarp();
+            unsigned const w0 = threadIdx.x - lane;
+            unsigned n = total / 4; // the words that fit in the arena (a lane that does not fit is redone)
+            if (wbase + total > p.arena_cap) n = wbase >= p.arena_cap ? 0 : (unsigned)((p.arena_cap - wbase) / 4);
+            unsigned const lead = (unsigned)(wbase / 4) & 31;
+            uint32_t *to = reinterpret_cast<uint32_t *>(p.arena + wbase) - lead;
+            uint32_t const *scratch = stage - (size_t)lane * kStageWords; // lane 0's
+            for (unsigned j = lane; j < n + lead; j += 32) {
+                if (j < lead) continue;
+                unsigned const i = j - lead;
+                unsigned l = 0;
+#pragma unroll
+                for (unsigned s = 16; s; s >>= 1)
+                    if (g_slice_seg[0][w0 + l + s] <= i) l += s;
+                unsigned const at = i - g_slice_seg[0][w0 + l];
+                uint32_t const v = i >= g_slice_seg[1][w0 + l] ? g_slice_win[at % kSliceWindow][w0 + l]
+                                                               : scratch[(size_t)l * kStageWords + at];
+                __stcs(to + j, v);
             }
-            if (active && (pass == 0 || (bytes && fits))) {
-                EventWriter w;
-                if (pass)
-                    w.init(reinterpret_cast<uint32_t *>(p.arena + off), bytes / 4, (unsigned)sp.gate);
-                else
-                    w.init(stage, stage_words, (unsigned)sp.gate);
-                slice_dispatch(pv, sp, w);
-                if (pass == 0) {
-                    bytes = w.committed * 4;
-                    nev = w.events;
-                    ng1 = w.gated1;
-                    ngN = w.gatedN;
-                }
-            }
+            __syncwarp();
+        } else if (active && bytes && fits) {
+            EventWriter w;
+            w.init(reinterpret_cast<uint32_t *>(p.arena + off), bytes / 4, (unsigned)sp.gate);
+            slice_dispatch(pv, sp, w);
         }
         if (active) {
             r433b_pair pr;

@@ -69,14 +69,49 @@ R4_HD uint32_t bswap32(uint32_t v)
 #endif
 }
 
+// k_slice2's write-combining window (Win = SliceWindow, r433b_kernels.cuh): the words at positions
+// [wb, wb + kSliceWindow) of a thread's output live in shared memory, Win::slot(at % kSliceWindow), and only whole
+// 32-byte sectors below the window reach `out`, the thread's scratch in global memory.  At least one sector; a power
+// of two so that the slot is a mask.  Tests build the emulator with a smaller one.
+#ifndef R4_SLICE_WINDOW
+#define R4_SLICE_WINDOW 16
+#endif
+constexpr unsigned kSliceWindow = R4_SLICE_WINDOW;
+static_assert(kSliceWindow >= 8 && (kSliceWindow & (kSliceWindow - 1)) == 0, "the window is a power of two of >= 1 sector");
+struct NoWindow { static constexpr bool kOn = false; };
+
+// The window moves forward to hold `at`: the sectors it leaves behind are written to `out` whole (slots of positions
+// never written carry stale words, which a later store behind the window or the copy-out never reads).  Returns the
+// new base.
+template <class Win>
+R4_HD unsigned window_slide(uint32_t *out, unsigned wb, unsigned at)
+{
+    unsigned const b = (at + 8 - kSliceWindow) & ~7u;
+    unsigned const end = b < wb + kSliceWindow ? b : wb + kSliceWindow;
+    for (unsigned s = wb; s < end; s += 8) {
+        uint32_t v[8];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) v[k] = Win::slot((s + k) % kSliceWindow);
+#ifdef __CUDA_ARCH__
+        reinterpret_cast<uint4 *>(out + s)[0] = make_uint4(v[0], v[1], v[2], v[3]);
+        reinterpret_cast<uint4 *>(out + s)[1] = make_uint4(v[4], v[5], v[6], v[7]);
+#else
+        for (int k = 0; k < 8; ++k) out[s + k] = v[k];
+#endif
+    }
+    return b;
+}
+
 // One writer type serves both passes: out == nullptr only counts.  All offsets are in 32-bit
-// words; every store is one aligned word.  Bits are gathered MSB-first in `acc` (bit i of the
-// row at position 31 - i%32) and byte-swapped on store, which yields bitbuffer_t's layout
+// words; every store is one aligned word (the window's: one sector).  Bits are gathered MSB-first in `acc` (bit i of
+// the row at position 31 - i%32) and byte-swapped on store, which yields bitbuffer_t's layout
 // (bit i in byte i/8 at position 7 - i%8) in little-endian memory.
-struct EventWriter {
+template <class Win = NoWindow>
+struct EventWriterT {
     uint32_t *out;      // pair region, or nullptr while counting
     unsigned limit;     // words the counting pass committed: rows of a trailing, never-emitted
                         // event lie beyond it and must not be written
+    unsigned wb;        // Win::kOn: window base, a multiple of 8; every position below it holds its latest value in `out`
 
     unsigned pos;       // words used by finished events + the current event so far
     unsigned committed; // words up to the end of the last emitted event
@@ -101,6 +136,7 @@ struct EventWriter {
     {
         out = o;
         limit = region_words;
+        wb = 0;
         pos = committed = 0;
         events = 0;
         gate = gate_bits;
@@ -119,11 +155,34 @@ struct EventWriter {
         acc = 0;
         dirty = false;
         max_bits = 0;
+        if constexpr (Win::kOn) {
+            if (committed < wb) { // rolled back below the window: it moves back to the sector holding `committed`
+                unsigned const b = committed & ~7u;
+                for (unsigned q = b; q < committed; ++q) Win::slot(q % kSliceWindow) = out[q];
+                wb = b;
+            }
+        }
     }
 
     R4_HD void put(unsigned at, uint32_t v)
     {
-        if (out && at < limit) out[at] = v;
+        if (!out || at >= limit) return;
+        if constexpr (Win::kOn) {
+            if (at >= wb + kSliceWindow) wb = window_slide<Win>(out, wb, at);
+            if (at >= wb) {
+                Win::slot(at % kSliceWindow) = v;
+                return;
+            }
+        }
+        out[at] = v;
+    }
+
+    R4_HD uint32_t get(unsigned at) const // a word this event already wrote
+    {
+        if constexpr (Win::kOn) {
+            if (at >= wb) return Win::slot(at % kSliceWindow);
+        }
+        return out[at];
     }
 
     R4_HD unsigned first_row_bits() const { return num_rows <= 1 ? bits : row0_bits; }
@@ -143,10 +202,8 @@ struct EventWriter {
         unsigned at = row_hdr + 1 + w;
         if (out && at < limit) {
             uint32_t v = bswap32(acc);
-            if (w < row_hw)
-                out[at] |= v;
-            else
-                out[at] = v;
+            if (w < row_hw) v |= get(at);
+            put(at, v);
         }
         if (w + 1 > row_hw) row_hw = w + 1;
         acc = 0;
@@ -262,6 +319,7 @@ struct EventWriter {
         reset_event();
     }
 };
+using EventWriter = EventWriterT<>;
 
 // ---------------------------------------------------------------------------- slicers ----
 
