@@ -275,21 +275,26 @@ __global__ void __launch_bounds__(kFrontWarps * 32, kFrontCtasPerSm) k_front(Fro
     bool run = true, fixed = false;
     for (;;) {
         if (run) {
+            if (fixed) {
+                // a chunk run again: its stage slot holds AM by now, so its IQ is staged again (L2 hits), every
+                // piece in flight at once (cp.async does not block), zero-filled past the stream end like the first time
+#pragma unroll 1
+                for (int q = 0; q < St::kChunkBytes / 16; ++q) {
+                    long long const smp = (long long)gpos + q * SPL;
+                    long long const left = (long long)N - smp;
+                    int const valid = left >= SPL ? 16 : (left > 0 ? (int)left * SS : 0);
+                    stage_piece(stage + St::at(base + q * SPL), valid ? src + smp * SS : src, valid);
+                }
+                stage_wait();
+            }
             int yy = ys, xx = xp_b;
             int k = 0;
-            // a chunk run again (`fixed`) reads its IQ from global memory: its stage slot holds AM by now
-            auto iq_at = [&](int kk, uint32_t (&rw)[4]) {
-                if (fixed)
-                    load_group<SS>(src, gpos + kk, (long long)N - (long long)(gpos + kk), p.flip, rw);
-                else
-                    group_at(base + kk, rw);
-            };
 #pragma unroll 2
             for (; k + SPL <= nv; k += SPL) {
                 uint32_t rw[4];
                 int x[SPL];
                 uint32_t o[SPL / 2];
-                iq_at(k, rw);
+                group_at(base + k, rw);
                 env_group<SS>(rw, p.use_mag, x);
 #pragma unroll
                 for (int j = 0; j < SPL; j += 2) {
@@ -318,7 +323,7 @@ __global__ void __launch_bounds__(kFrontWarps * 32, kFrontCtasPerSm) k_front(Fro
             if (k < nv) { // ragged end of the stream (the stage is zero-filled past it)
                 uint32_t rw[4];
                 int x[SPL];
-                iq_at(k, rw);
+                group_at(base + k, rw);
                 env_group<SS>(rw, p.use_mag, x);
 #pragma unroll
                 for (int j = 0; j < SPL; ++j) {
