@@ -122,6 +122,8 @@ typedef struct r433b_timing {
     uint32_t front_launches;
     uint32_t front_redone;   /* 64-sample chunks k_front ran twice (its guess of the filter state did not verify) */
     uint32_t front_repairs;  /* tiles whose start k_detect recomputed (k_front's guess for the tile did not fit) */
+    uint32_t idle_skipped;   /* IDLE tiles k_detect ruled out from their summaries without walking them */
+    uint32_t idle_rewalks;   /* runs of such tiles walked again because their end state could not be resolved */
 } r433b_timing;
 
 int r433b_create(int cuda_device, r433b_ctx **out);

@@ -67,7 +67,7 @@ struct r433b_ctx {
     unsigned fpdm = 0;
     int enable_fm = 0;
     int n_sms = 132;        // cudaDevAttrMultiProcessorCount of `device`
-    int spoil_front = 0; // R433B_SPOIL_FRONT=1|2: k_front starts from wrong guesses (tests of the redo / repair paths)
+    int spoil_front = 0; // R433B_SPOIL_FRONT=1|2|3: k_front starts from wrong guesses (tests of the redo / repair paths)
     Levels lv{};
     // device memory (grow only)
     DevBuf d_data, d_offsets, d_train, d_pkgs, d_ppool, d_gpool, d_counters, d_am, d_fm;
@@ -87,7 +87,7 @@ struct r433b_ctx {
     static constexpr int kMaxGroups = 16;
     cudaEvent_t ev_in[kMaxGroups]{}, ev_det[kMaxGroups]{}, ev_slc[kMaxGroups]{}, ev_t[4 * kMaxGroups]{}, ev_f[kMaxGroups]{}, ev_init = nullptr;
     DevBuf d_order; // k_bucket: package indices sorted by (type, length class), per range
-    DevBuf d_ranges, d_state, d_lengths, d_stage, d_raw, d_log, d_amoff, d_chunks;
+    DevBuf d_ranges, d_state, d_lengths, d_stage, d_raw, d_log, d_amoff, d_chunks, d_tiles;
     std::vector<uint64_t> am_offsets; // first sample of stream i in d_am (multiples of the tile), n_streams + 1
     HostBuf h_ranges;
     bool d2h_done = false;
@@ -221,7 +221,7 @@ void r433b_destroy(r433b_ctx *ctx)
     cudaSetDevice(ctx->device);
     for (DevBuf *b : {&ctx->d_data, &ctx->d_offsets, &ctx->d_train, &ctx->d_pkgs, &ctx->d_ppool, &ctx->d_gpool,
                  &ctx->d_counters, &ctx->d_am, &ctx->d_fm, &ctx->d_devparams, &ctx->d_lists, &ctx->d_pairs,
-                 &ctx->d_arena, &ctx->d_cursor, &ctx->d_ranges, &ctx->d_state, &ctx->d_lengths, &ctx->d_stage, &ctx->d_raw, &ctx->d_log, &ctx->d_amoff, &ctx->d_chunks,
+                 &ctx->d_arena, &ctx->d_cursor, &ctx->d_ranges, &ctx->d_state, &ctx->d_lengths, &ctx->d_stage, &ctx->d_raw, &ctx->d_log, &ctx->d_amoff, &ctx->d_chunks, &ctx->d_tiles,
                  &ctx->d_order, &ctx->d_an, &ctx->d_an_dev, &ctx->d_an_gap, &ctx->d_an_pairs, &ctx->d_an_arena})
         if (b->p) cudaFree(b->p);
     for (HostBuf *b : {&ctx->h_pkgs, &ctx->h_ppool, &ctx->h_gpool, &ctx->h_pairs, &ctx->h_events, &ctx->h_ranges})
@@ -486,6 +486,7 @@ int r433b_process(r433b_ctx *ctx, r433b_batch const *b)
     uint64_t const am_samples = ctx->am_offsets[b->n_streams];
     if (int r = dev_reserve(ctx, ctx->d_am, am_samples * sizeof(int16_t) + 16)) return r;
     if (int r = dev_reserve(ctx, ctx->d_chunks, am_samples / kChunk * sizeof(ChunkInfo) + 16)) return r;
+    if (int r = dev_reserve(ctx, ctx->d_tiles, am_samples / T * sizeof(TileInfo) + 16)) return r;
     if (int r = dev_reserve(ctx, ctx->d_amoff, (b->n_streams + 1) * sizeof(uint64_t))) return r;
     CU(cudaMemcpy(ctx->d_amoff.p, ctx->am_offsets.data(), (b->n_streams + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice));
     if (b->want_stages)
@@ -525,6 +526,7 @@ int r433b_process(r433b_ctx *ctx, r433b_batch const *b)
     dp.am_offsets = (unsigned long long const *)ctx->d_amoff.p;
     dp.am = (int16_t *)ctx->d_am.p;
     dp.chunks = (ChunkInfo const *)ctx->d_chunks.p;
+    dp.tile_info = (TileInfo const *)ctx->d_tiles.p;
     dp.want_stages = b->want_stages ? 1 : 0;
     dp.fm_out = b->want_stages ? (int16_t *)ctx->d_fm.p : nullptr;
 
@@ -551,6 +553,7 @@ int r433b_process(r433b_ctx *ctx, r433b_batch const *b)
             fp.b0 = q.lpf_b0;
             fp.am = q.am;
             fp.chunks = (ChunkInfo *)ctx->d_chunks.p;
+            fp.tile_info = (TileInfo *)ctx->d_tiles.p;
             fp.counters = q.counters;
             fp.spoil = ctx->spoil_front;
             uint64_t const warps = (uint64_t)q.n_streams * fp.tiles;
@@ -718,6 +721,8 @@ int r433b_process(r433b_ctx *ctx, r433b_batch const *b)
             CU(cudaMemcpy(stat, ctx->d_counters.p, sizeof(stat), cudaMemcpyDeviceToHost));
             ctx->timing.front_redone = stat[4];
             ctx->timing.front_repairs = stat[5];
+            ctx->timing.idle_skipped = stat[6];
+            ctx->timing.idle_rewalks = stat[7];
             ctx->timing.h2d_ms = 0; // overlapped: only the wall total is meaningful
             ctx->timing.d2h_ms = 0;
             ctx->timing.detect_ms = det;
@@ -796,6 +801,8 @@ int r433b_process(r433b_ctx *ctx, r433b_batch const *b)
     ctx->timing.front_launches = detect_launches;
     ctx->timing.front_redone = counters[4];
     ctx->timing.front_repairs = counters[5];
+    ctx->timing.idle_skipped = counters[6];
+    ctx->timing.idle_rewalks = counters[7];
     cudaEventElapsedTime(&ctx->timing.total_ms, ctx->ev[0], ctx->ev[3]);
     ctx->timing.d2h_ms = 0;
     ctx->timing.detect_launches = detect_launches;

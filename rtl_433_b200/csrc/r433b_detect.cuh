@@ -9,6 +9,8 @@
 //     step(last AM of the previous tile, x[-1], x[0]) equals the first stored AM of this one.  If not (rare),
 //     the walk recomputes forward from the exact state until its values meet the stored ones again; from
 //     there on the stored values are the exact ones (k_front's chunks are consistent with each other).
+//     In IDLE, whole noise tiles are ruled out from k_front's tile summaries before any of this (idle_skip):
+//     their AM is never loaded.
 //
 //  2. The package detector (src/pulse_detect.c:199-483) walks the tile warp-uniformly with ballot scans for
 //     the states whose thresholds are frozen (IDLE stretches by bracket rounds, GAP, GAP_START) and a
@@ -66,12 +68,12 @@ constexpr int kF1Tail = R4_F1_TAIL;        // samples of the first evaluation at
 struct FmJob {
     uint8_t const *src;        // the stream
     unsigned long long N;      // its length in samples
-    unsigned flip;
     long long a1, b0;
+    int16_t *fm_out;           // stage dump (absolute index = stream base + sample) or nullptr
+    unsigned flip;
     int fm_on;                 // 0: "FM" is the raw envelope (buf.fm aliases buf.temp when nothing asks for FM)
     int use_mag;
     int monotone;              // the state rebuild by range collapse is valid
-    int16_t *fm_out;           // stage dump (absolute index = stream base + sample) or nullptr
 };
 
 // Warp-uniform state of the walk.  It lives in shared memory BETWEEN the phases of the walk (idle_run, burst_run,
@@ -82,9 +84,11 @@ struct WalkState {
     unsigned log_n, log_start, log_count; // deferred carrier-estimate log: closed entries (global memory), the open entry
     unsigned seq;
     int pend_type;               // a finished package to hand over (1 OOK, 2 FSK) ...
+    int skip_y;                  // idle_skip: the AM filter state in front of the tile it returns
     unsigned long long pend_pos; // ... returned at this stream position
     unsigned long long t0;       // the tile being walked
     int nv_tile;
+    unsigned rewalk_end;         // idle_skip: tiles (index) in front of this one are walked without skipping (a run walked again)
 };
 
 // Per-stream constants of the walk (written once by lane 0)
@@ -99,6 +103,7 @@ struct WalkConst {
     int *pulse_pool, *gap_pool;
     unsigned pkg_cap, pool_cap;
     unsigned *counters;
+    TileInfo const *tiles;       // the stream's tile summaries; nullptr: no tile is skipped (idle_skip)
 };
 
 // Shared memory of one warp
@@ -157,6 +162,7 @@ struct DetectParams {
     unsigned *counters; // [0] packages, [1] pool entries, [2] overflow flag, [4..] statistics
     int16_t *am;               // k_front's output (repaired in place where a tile did not fit its predecessor)
     ChunkInfo const *chunks;   // bounds of every 64-sample chunk of `am`
+    TileInfo const *tile_info; // summary of every tile of `am` (as k_front made it: never updated by a repair)
     int16_t *fm_out;           // optional stage dump, indexed by offsets[s]/SS + n
 };
 
@@ -694,136 +700,141 @@ __device__ R4_NOINLINE void walk_emit(WarpSmem &sm, int type, unsigned long long
 
 __device__ __forceinline__ int am_tile_at(uint16_t const *am16, int n) { return (int)am16[(n >> 6) * (2 * kAmStride) + (n & 63)]; }
 
-// IDLE from tile sample n on: only the noise-floor tracker moves.  Returns the first sample it could not take
-// (a trigger is conceivable there, or the tracker leaves its +-1 regime): the generic step looks at that one.
-__device__ R4_NOINLINE int idle_run(WarpSmem &sm, int n)
+// the IDLE state the noise-floor tracker phases carry in registers
+struct IdleRegs {
+    int low, high, lead_in;
+};
+
+// IDLE over a long stretch of the tile in sm.am from sample n on, lane-parallel: see the comment in the file header
+// and below.  While |am - low| < 1024 the tracker is low += (am > low) ? +1 : -1, so low keeps the parity of
+// (low0 + samples seen) and two trajectories of equal parity never cross and merge once the data passes between
+// them: lane l takes chunk l, starts from a bracket [lo, hi] of the right parity that provably contains the true
+// value, pushes both ends through its chunk and hands them to the next lane until the bracket at the end of the
+// stretch has collapsed.  Chunks in which a trigger is conceivable (or |am - low| could reach 1024) end the stretch.
+// [lo0, hi0] holds the tracker value in front of sample n and has its parity (lo0 == hi0 == d.low when it is known
+// exactly; idle_skip starts from a bracket).  `high` must have been derived from `low` already.  Returns the samples
+// taken (0: none); d then holds the exact state behind them.
+__device__ __forceinline__ int idle_tile(WarpSmem const &sm, IdleRegs &d, int n, int lo0, int hi0, Levels const &lv, int nv_tile)
 {
     constexpr int C = kChunk;
     int const lane = threadIdx.x & 31;
     uint16_t const *am16 = reinterpret_cast<uint16_t const *>(sm.am);
+    if (nv_tile - n < 2 * C) return 0;
+    int const c0 = n / C;
+    int const k0 = lane == c0 ? n - c0 * C : 0;
+    int k1 = nv_tile - lane * C;
+    k1 = k1 > C ? C : k1;
+    bool const in_region = lane >= c0 && k1 > k0;
+    // bounds of the chunk's AM values (of the whole chunk for the first, partial one: still bounds)
+    int const cmin = in_region ? sm.cmin[lane] : 32767, cmax = in_region ? sm.cmax[lane] : -32768;
+    int pmin = cmin, pmax = cmax; // over chunks c0..lane
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        int t1 = __shfl_up_sync(0xffffffffu, pmin, o);
+        int t2 = __shfl_up_sync(0xffffffffu, pmax, o);
+        if (lane >= o) {
+            pmin = t1 < pmin ? t1 : pmin;
+            pmax = t2 > pmax ? t2 : pmax;
+        }
+    }
+    int Lmin = lo0 < pmin - 1 ? lo0 : pmin - 1;
+    int Lmax = hi0 > pmax ? hi0 : pmax;
+    int hmin = lv.ratio * Lmin;
+    if (hmin < lv.min_high) hmin = lv.min_high;
+    Thresholds th = det_thresholds(Lmin, hmin, lv);
+    bool const armed = d.lead_in + (nv_tile - n) > kLeadIn;
+    bool ok = in_region && !(armed && cmax > th.up) && (pmax - Lmin < 1024) && (Lmax - pmin < 1024);
+    unsigned bad = ~__ballot_sync(0xffffffffu, ok) & (0xffffffffu << c0);
+    int const e = bad ? __ffs(bad) - 1 : 32; // chunks c0 .. e-1 form the stretch
+    if (e - c0 < 2) return 0;
+    int const RLmin = __shfl_sync(0xffffffffu, Lmin, e - 1);
+    int const RLmax = __shfl_sync(0xffffffffu, Lmax, e - 1);
+    bool const act = lane >= c0 && lane < e;
+    int const par = (lo0 + (lane * C + k0 - n)) & 1; // parity of the true value at this lane's start
+    // Start bracket.  Over K samples whose values lie in [m, M] the tracker climbs one per sample
+    // until it is >= m - 1 and falls one per sample until it is <= M, so from any start in [A, B] it
+    // ends in [min(A + K, m - 1), max(B - K, M)].  The chunk to the left has K = 64 samples (the first
+    // chunk of the stretch may be partial: then the start bracket and its real length are used).
+    int m1 = __shfl_up_sync(0xffffffffu, cmin, 1), M1 = __shfl_up_sync(0xffffffffu, cmax, 1);
+    int K1 = __shfl_up_sync(0xffffffffu, k1 - k0, 1);
+    int lo, hi;
+    if (lane == c0 + 1) {
+        lo = lo0 + K1 < m1 - 1 ? lo0 + K1 : m1 - 1;
+        hi = hi0 - K1 > M1 ? hi0 - K1 : M1;
+    } else {
+        lo = RLmin + K1 < m1 - 1 ? RLmin + K1 : m1 - 1;
+        hi = RLmax - K1 > M1 ? RLmax - K1 : M1;
+    }
+    lo = lo < RLmin ? RLmin : lo;
+    hi = hi > RLmax ? RLmax : hi;
+    lo -= (lo - par) & 1;
+    hi += (hi - par) & 1;
+    if (lane == c0) {
+        lo = lo0;
+        hi = hi0;
+    }
+    uint16_t const *chunk = am16 + lane * (2 * kAmStride);
+    int result = 0;
+    bool done = false;
+#pragma unroll 1
+    for (int round = 0; round < 6; ++round) {
+        int elo = lo, ehi = hi;
+        if (act) {
+            if (elo == ehi) {
+#pragma unroll 2
+                for (int k = k0; k < k1; ++k) elo += (int)chunk[k] > elo ? 1 : -1;
+                ehi = elo;
+            } else {
+#pragma unroll 2
+                for (int k = k0; k < k1; ++k) {
+                    int a = (int)chunk[k];
+                    elo += a > elo ? 1 : -1;
+                    ehi += a > ehi ? 1 : -1;
+                }
+            }
+        }
+        // the true value lies inside every bracket: a collapsed end bracket is the true value (the first chunk's
+        // may never collapse when it starts from a bracket; the last one's decides)
+        if (__shfl_sync(0xffffffffu, elo == ehi, e - 1)) {
+            result = __shfl_sync(0xffffffffu, elo, e - 1);
+            done = true;
+            break;
+        }
+        int nlo = __shfl_up_sync(0xffffffffu, elo, 1);
+        int nhi = __shfl_up_sync(0xffffffffu, ehi, 1);
+        if (act && lane != c0) {
+            lo = nlo;
+            hi = nhi;
+        }
+    }
+    if (!done) return 0;
+    int const len = (e * C < nv_tile ? e * C : nv_tile) - n;
+    d.low = result;
+    int hh = lv.ratio * d.low;
+    d.high = hh < lv.min_high ? lv.min_high : hh;
+    int li = d.lead_in + len;
+    d.lead_in = li > kLeadIn + 1 ? kLeadIn + 1 : li;
+    return len;
+}
+
+// IDLE from tile sample n on: only the noise-floor tracker moves.  Returns the first sample it could not take
+// (a trigger is conceivable there, the tracker leaves its +-1 regime, or `high` has not been re-derived from `low`
+// yet after a package): the generic step looks at that one.
+__device__ R4_NOINLINE int idle_run(WarpSmem &sm, int n)
+{
+    int const lane = threadIdx.x & 31;
+    uint16_t const *am16 = reinterpret_cast<uint16_t const *>(sm.am);
     __syncwarp();
-    struct {
-        int low, high, lead_in;
-    } d = {sm.ws.d.low, sm.ws.d.high, sm.ws.d.lead_in};
+    IdleRegs d = {sm.ws.d.low, sm.ws.d.high, sm.ws.d.lead_in};
     Levels const lv = sm.wc.lv;
     int const nv_tile = sm.ws.nv_tile;
     auto am_at = [&](int i) -> int { return am_tile_at(am16, i); };
-
-    // IDLE over a long stretch, lane-parallel: see the comment in the file header and below.
-    // While |am - low| < 1024 the tracker is low += (am > low) ? +1 : -1, so low keeps the parity of
-    // (low0 + samples seen) and two trajectories of equal parity never cross and merge once the data
-    // passes between them: lane l takes chunk l, starts from a bracket [lo, hi] of the right parity that
-    // provably contains the true value, pushes both ends through its chunk and hands them to the next
-    // lane until every bracket has collapsed.  Chunks in which a trigger is conceivable (or
-    // |am - low| could reach 1024) end the stretch.
-    auto idle_tile = [&](int n) -> int {
-        if (nv_tile - n < 2 * C) return 0;
-        {
-            int hs = lv.ratio * d.low;
-            if (hs < lv.min_high) hs = lv.min_high;
-            if (d.high != hs) return 0;
-        }
-        int const c0 = n / C;
-        int const k0 = lane == c0 ? n - c0 * C : 0;
-        int k1 = nv_tile - lane * C;
-        k1 = k1 > C ? C : k1;
-        bool const in_region = lane >= c0 && k1 > k0;
-        // bounds of the chunk's AM values (of the whole chunk for the first, partial one: still bounds)
-        int const cmin = in_region ? sm.cmin[lane] : 32767, cmax = in_region ? sm.cmax[lane] : -32768;
-        int pmin = cmin, pmax = cmax; // over chunks c0..lane
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            int t1 = __shfl_up_sync(0xffffffffu, pmin, o);
-            int t2 = __shfl_up_sync(0xffffffffu, pmax, o);
-            if (lane >= o) {
-                pmin = t1 < pmin ? t1 : pmin;
-                pmax = t2 > pmax ? t2 : pmax;
-            }
-        }
-        int Lmin = d.low < pmin - 1 ? d.low : pmin - 1;
-        int Lmax = d.low > pmax ? d.low : pmax;
-        int hmin = lv.ratio * Lmin;
-        if (hmin < lv.min_high) hmin = lv.min_high;
-        Thresholds th = det_thresholds(Lmin, hmin, lv);
-        bool const armed = d.lead_in + (nv_tile - n) > kLeadIn;
-        bool ok = in_region && !(armed && cmax > th.up) && (pmax - Lmin < 1024) && (Lmax - pmin < 1024);
-        unsigned bad = ~__ballot_sync(0xffffffffu, ok) & (0xffffffffu << c0);
-        int const e = bad ? __ffs(bad) - 1 : 32; // chunks c0 .. e-1 form the stretch
-        if (e - c0 < 2) return 0;
-        int const RLmin = __shfl_sync(0xffffffffu, Lmin, e - 1);
-        int const RLmax = __shfl_sync(0xffffffffu, Lmax, e - 1);
-        bool const act = lane >= c0 && lane < e;
-        int const par = (d.low + (lane * C + k0 - n)) & 1; // parity of the true value at this lane's start
-        // Start bracket.  Over K samples whose values lie in [m, M] the tracker climbs one per sample
-        // until it is >= m - 1 and falls one per sample until it is <= M, so from any start in [A, B] it
-        // ends in [min(A + K, m - 1), max(B - K, M)].  The chunk to the left has K = 64 samples (the first
-        // chunk of the stretch may be partial: then the exact start value and its real length are used).
-        int m1 = __shfl_up_sync(0xffffffffu, cmin, 1), M1 = __shfl_up_sync(0xffffffffu, cmax, 1);
-        int K1 = __shfl_up_sync(0xffffffffu, k1 - k0, 1);
-        int lo, hi;
-        if (lane == c0 + 1) {
-            lo = d.low + K1 < m1 - 1 ? d.low + K1 : m1 - 1;
-            hi = d.low - K1 > M1 ? d.low - K1 : M1;
-        } else {
-            lo = RLmin + K1 < m1 - 1 ? RLmin + K1 : m1 - 1;
-            hi = RLmax - K1 > M1 ? RLmax - K1 : M1;
-        }
-        lo = lo < RLmin ? RLmin : lo;
-        hi = hi > RLmax ? RLmax : hi;
-        lo -= (lo - par) & 1;
-        hi += (hi - par) & 1;
-        if (lane == c0) lo = hi = d.low;
-        uint16_t const *chunk = am16 + lane * (2 * kAmStride);
-        int result = 0;
-        bool done = false;
-#pragma unroll 1
-        for (int round = 0; round < 6; ++round) {
-            int elo = lo, ehi = hi;
-            if (act) {
-                if (elo == ehi) {
-#pragma unroll 2
-                    for (int k = k0; k < k1; ++k) elo += (int)chunk[k] > elo ? 1 : -1;
-                    ehi = elo;
-                } else {
-#pragma unroll 2
-                    for (int k = k0; k < k1; ++k) {
-                        int a = (int)chunk[k];
-                        elo += a > elo ? 1 : -1;
-                        ehi += a > ehi ? 1 : -1;
-                    }
-                }
-            }
-            // the true value lies inside every bracket: collapsed end brackets are the true values
-            if (__all_sync(0xffffffffu, !act || elo == ehi)) {
-                result = __shfl_sync(0xffffffffu, elo, e - 1);
-                done = true;
-                break;
-            }
-            int nlo = __shfl_up_sync(0xffffffffu, elo, 1);
-            int nhi = __shfl_up_sync(0xffffffffu, ehi, 1);
-            if (act && lane != c0) {
-                lo = nlo;
-                hi = nhi;
-            }
-        }
-        if (!done) return 0;
-        int const len = (e * C < nv_tile ? e * C : nv_tile) - n;
-        d.low = result;
-        int hh = lv.ratio * d.low;
-        d.high = hh < lv.min_high ? lv.min_high : hh;
-        int li = d.lead_in + len;
-        d.lead_in = li > kLeadIn + 1 ? kLeadIn + 1 : li;
-        return len;
-    };
 
     // IDLE: only the noise-floor tracker moves (src/pulse_detect.c:325-334).  While
     // |am - low| < 1024 it is low += (am > low) ? +1 : -1; with q = low + j that is
     // q += 2 * (am_j + j > q): two dependent instructions per sample.
     auto idle_fast = [&](int n) -> int {
         int cnt = nv_tile - n < 32 ? nv_tile - n : 32;
-        int hs = lv.ratio * d.low;
-        if (hs < lv.min_high) hs = lv.min_high;
-        if (d.high != hs) return 0; // first IDLE sample after a package: not yet re-derived
         int a = lane < cnt ? am_at(n + lane) : -32768;
         int lmin = d.low - cnt;
         int hmin = lv.ratio * lmin;
@@ -863,7 +874,10 @@ __device__ R4_NOINLINE int idle_run(WarpSmem &sm, int n)
 
 
     while (n < nv_tile) {
-        int adv = idle_tile(n);
+        int hs = lv.ratio * d.low;
+        if (hs < lv.min_high) hs = lv.min_high;
+        if (d.high != hs) break; // first IDLE sample after a package: not yet re-derived
+        int adv = idle_tile(sm, d, n, d.low, d.low, lv, nv_tile);
         if (!adv) adv = idle_fast(n);
         if (!adv) break;
         n += adv;
@@ -876,6 +890,133 @@ __device__ R4_NOINLINE int idle_run(WarpSmem &sm, int n)
     }
     __syncwarp();
     return n;
+}
+
+// Whole IDLE tiles ruled out from k_front's tile summaries, without loading their AM.  Called at the top of the tile
+// at t0 in IDLE with `high` derived from `low` (and no package pending); y_am is the exact AM filter state in front
+// of t0.  Lane l looks at tile t0 + l of up to 32 tiles per pass.  Tile j is skipped when
+//   * it continues tile j - 1: step(last AM of j - 1, x[0] + x[-1]) is its first stored AM.  Lane 0 takes the walk's
+//     exact y_am; the others the summary of tile j - 1, which was skipped too and so holds exact AM by induction.
+//     k_front's tile is consistent from its first value on, so tile j's stored AM is exact and its summary bounds are
+//     real bounds;
+//   * the tracker stays in its +-1 regime and no trigger is conceivable anywhere in it: idle_tile's conditions on the
+//     whole tile, from the tracker's bracket in front of it.  That is the walk's [lo, hi] on lane 0.  Behind a skipped
+//     tile with values in [m, M] it is [m - 1, M] (idle_tile's [min(A + K, m - 1), max(B - K, M)] with K = 2048: the
+//     regime conditions keep A, B within 1024 of the values), cut to the parity of `low` in front of t0 (a tile is
+//     2048 samples: the parity at every tile start is the same);
+//   * it is not the last tile of the launch's range, so a launch always ends on a walked tile (and StreamState holds
+//     exact values).
+// The prefix of skipped tiles is taken with one ballot.  A block start inside it is a no-op for this state: the call
+// boundary clamps `high` to min_high, which a derived `high` already respects, and clears eop_flag, which is zero in
+// IDLE (a set flag ends its package at the next sample).
+// The exact `low` behind the run is recovered from the last skipped tile's AM by idle_tile's bracket rounds, started
+// from the bracket in front of that tile.  Should they not collapse, the run is walked again tile by tile from the
+// exact state it started from, up to ws.rewalk_end.  Returns the tile to walk next; ws.skip_y is the AM filter state in
+// front of it, ws.d the exact detector state.
+#ifndef R4_FORCE_REWALK
+#define R4_FORCE_REWALK 0 // tests: 1 = no skipped run is resolved by bracket rounds, every one is walked again
+#endif
+__device__ R4_NOINLINE unsigned long long idle_skip(WarpSmem &sm, int16_t const *am_stream, ChunkInfo const *chunk_stream,
+        unsigned long long t0, unsigned long long sample_end, int y_am, int a1, int b0)
+{
+    constexpr int T = kTile;
+    int const lane = threadIdx.x & 31;
+    __syncwarp();
+    Levels const lv = sm.wc.lv;
+    TileInfo const *const tiles = sm.wc.tiles;
+    unsigned long long const range_end = sample_end < sm.wc.jb.N ? sample_end : sm.wc.jb.N; // end of the launch's range
+    int const low0 = sm.ws.d.low, lead0 = sm.ws.d.lead_in;
+    int const par = low0 & 1;
+    int lo = low0, hi = low0, lead = lead0, y = y_am; // in front of tile t
+    int plo = 0, phi = 0, plead = 0;                  // in front of the last skipped tile
+    unsigned long long t = t0;
+#pragma unroll 1
+    for (;;) {
+        unsigned long long const tl = t + (unsigned long long)lane * T;
+        bool const inside = tl + T < range_end;
+        TileInfo const ti = inside ? tiles[tl / T] : TileInfo{};
+        int const tmin = ti.tmin, tmax = ti.tmax, last = ti.last;
+        int const pmin = __shfl_up_sync(0xffffffffu, tmin, 1);
+        int const pmax = __shfl_up_sync(0xffffffffu, tmax, 1);
+        int const plast = __shfl_up_sync(0xffffffffu, last, 1);
+        int blo = pmin - 1, bhi = pmax; // the tracker's bracket in front of this tile
+        blo += (blo - par) & 1;
+        bhi -= (bhi - par) & 1;
+        int yin = plast;
+        if (lane == 0) {
+            blo = lo;
+            bhi = hi;
+            yin = y;
+        }
+        int li = lead + lane * T;
+        li = li > kLeadIn + 1 ? kLeadIn + 1 : li;
+        int const Lmin = blo < tmin - 1 ? blo : tmin - 1;
+        int const Lmax = bhi > tmax ? bhi : tmax;
+        int hmin = lv.ratio * Lmin;
+        if (hmin < lv.min_high) hmin = lv.min_high;
+        bool const armed = li + T > kLeadIn;
+        bool const ok = inside && iir16_nowrap(yin, a1, b0, ti.xsum) == (int)ti.first && tmax - Lmin < 1024
+                && Lmax - tmin < 1024 && !(armed && tmax > det_thresholds(Lmin, hmin, lv).up);
+        unsigned const bad = ~__ballot_sync(0xffffffffu, ok);
+        int const e = bad ? __ffs(bad) - 1 : 32; // tiles t .. t + e - 1 are skipped
+        if (e == 0) break;
+        plo = __shfl_sync(0xffffffffu, blo, e - 1);
+        phi = __shfl_sync(0xffffffffu, bhi, e - 1);
+        plead = __shfl_sync(0xffffffffu, li, e - 1);
+        int xlo = tmin - 1, xhi = tmax; // behind this tile
+        xlo += (xlo - par) & 1;
+        xhi -= (xhi - par) & 1;
+        lo = __shfl_sync(0xffffffffu, xlo, e - 1);
+        hi = __shfl_sync(0xffffffffu, xhi, e - 1);
+        y = __shfl_sync(0xffffffffu, last, e - 1);
+        lead = plead + T > kLeadIn + 1 ? kLeadIn + 1 : plead + T;
+        t += (unsigned long long)e * T;
+        if (e < 32) break;
+    }
+    if (t != t0) {
+        // the exact tracker value behind the run, from the last skipped tile's AM
+        unsigned long long const tp = t - T;
+        {
+            uint4 const *g = reinterpret_cast<uint4 const *>(am_stream + tp + (unsigned long long)(lane * kChunk));
+            uint4 v[8];
+#pragma unroll
+            for (int i = 0; i < 8; ++i) v[i] = g[i];
+            ChunkInfo const ci = chunk_stream[tp / kChunk + lane];
+            uint32_t *const mine = sm.am + lane * kAmStride;
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+                mine[4 * i + 0] = v[i].x;
+                mine[4 * i + 1] = v[i].y;
+                mine[4 * i + 2] = v[i].z;
+                mine[4 * i + 3] = v[i].w;
+            }
+            sm.cmin[lane] = ci.cmin;
+            sm.cmax[lane] = ci.cmax;
+            __syncwarp();
+        }
+        IdleRegs d = {plo, 0, plead};
+        int const len = R4_FORCE_REWALK ? 0 : idle_tile(sm, d, 0, plo, phi, lv, T);
+        __syncwarp();
+        if (len == T) {
+            if (lane == 0) {
+                sm.ws.d.low = d.low;
+                sm.ws.d.high = d.high;
+                sm.ws.d.lead_in = d.lead_in;
+                sm.ws.skip_y = y;
+                atomicAdd(&sm.wc.counters[6], (unsigned)((t - t0) / T));
+            }
+            __syncwarp();
+            return t;
+        }
+        // not resolved: the run is walked again from t0 (ws.d still holds the exact state there)
+        if (lane == 0) {
+            sm.ws.rewalk_end = (unsigned)(t / T);
+            atomicAdd(&sm.wc.counters[7], 1u);
+        }
+    }
+    if (lane == 0) sm.ws.skip_y = y_am;
+    __syncwarp();
+    return t0;
 }
 
     // Everything of a package after its first pulse (and the first real gap), in one loop with the hot
@@ -1312,11 +1453,15 @@ __global__ void __launch_bounds__(kDetectWarps * 32, kDetectCtasPerSm) k_detect(
         wc.pkg_cap = p.pkg_cap;
         wc.pool_cap = p.pool_cap;
         wc.counters = p.counters;
+        // idle tiles are skipped when nothing but the tracker needs them: no FM made for every tile, no stage dump
+        wc.tiles = lazy_fm && !p.fm_out ? p.tile_info + p.am_offsets[s] / kTile : nullptr;
         WalkState &ws = sm.ws;
         ws.pend_type = 0;
         ws.pend_pos = 0;
         ws.t0 = 0;
         ws.nv_tile = 0;
+        ws.skip_y = 0;
+        ws.rewalk_end = 0;
         if (p.first_chunk) {
             det_reset(ws.d);
             ws.d.ook_hw = ws.d.fsk_hw = kMaxPulses; // scratch is not assumed to be zero: first package clears it
@@ -1347,6 +1492,14 @@ __global__ void __launch_bounds__(kDetectWarps * 32, kDetectCtasPerSm) k_detect(
     int const a1 = p.lpf_a1, b0 = p.lpf_b0;
 
     for (unsigned long long t0 = p.sample_begin; t0 < p.sample_end && t0 < N; t0 += T) {
+        if (sm.wc.tiles && sm.ws.d.st == kIdle && !sm.ws.pend_type && !sm.ws.d.eop_flag && t0 / T >= sm.ws.rewalk_end) {
+            int hs = p.lv.ratio * sm.ws.d.low;
+            if (hs < p.lv.min_high) hs = p.lv.min_high;
+            if (sm.ws.d.high == hs) {
+                t0 = idle_skip(sm, am_stream, chunk_stream, t0, p.sample_end, y_am, a1, b0);
+                y_am = sm.ws.skip_y;
+            }
+        }
         unsigned long long const remain = N - t0;
         int const nv_tile = remain < (unsigned long long)T ? (int)remain : T;
 

@@ -47,6 +47,16 @@ struct ChunkInfo {
     int16_t cmin, cmax;
 };
 
+// Summary of one tile, enough for k_detect to rule a noise tile out without loading its AM (r433b_detect.cuh,
+// idle_skip): bounds of the stored AM (wider than the truth or exact, never narrower), the stored AM of its first
+// and last sample, and x[0] + x[-1] as the hand-over check feeds the filter (x[-1] narrowed at block starts).
+struct alignas(16) TileInfo {
+    int16_t tmin, tmax;
+    int16_t first, last;
+    int32_t xsum;
+    int32_t pad;
+};
+
 // 16 contiguous bytes (8 cu8 / 4 cs16 samples) starting at sample `pos` of the stream: one 128-bit load;
 // zero-filled past `n_valid` samples counted from pos.
 template <int SS>
@@ -145,8 +155,10 @@ struct FrontParams {
     int a1, b0;
     int16_t *am;
     ChunkInfo *chunks;                    // one per 64 samples of `am`
+    TileInfo *tile_info;                  // one per tile of `am`
     unsigned *counters;                   // [4] chunks done twice
-    int spoil;                            // tests: 1 = lane 0's guess is made wrong, 2 = every lane's (R433B_SPOIL_FRONT)
+    int spoil;                            // tests: 1 = lane 0's guess is made wrong, 2 = every lane's, 3 = lane 0's in every
+                                          // 7th tile (R433B_SPOIL_FRONT)
 };
 
 // Shared-memory staging of one tile's IQ: the chunks [-kWarmChunks, 32) of the tile, every chunk (C samples)
@@ -259,6 +271,15 @@ __global__ void __launch_bounds__(kFrontWarps * 32, kFrontCtasPerSm) k_front(Fro
             }
         }
     }
+    // x[0] of the tile, for the tile summary
+    int x0;
+    {
+        uint32_t rw[4];
+        int x[SPL];
+        group_at(0, rw);
+        env_group<SS>(rw, p.use_mag, x);
+        x0 = x[0];
+    }
     // From here on a lane's AM overwrites its own chunk's IQ in the stage (no other lane reads that chunk again), and
     // the warp stores the whole tile at the end, whole lines per instruction.  Stored lane by lane (32 partial lines
     // 128 bytes apart per instruction), the tiles in flight overflow the 50 MB L2 of an H100.
@@ -266,7 +287,9 @@ __global__ void __launch_bounds__(kFrontWarps * 32, kFrontCtasPerSm) k_front(Fro
     // the reference keeps x[-1] as int16 across block calls (src/baseband.c:167): only the first sample of a
     // block sees the narrowed value, and block starts are tile starts
     if (gpos % p.block_samples == 0) xp = (int)(int16_t)xp;
-    if (p.spoil && gpos != 0 && (lane == 0 || p.spoil > 1)) y = y > 16000 ? y - 999 : y + 999; // tests: force the redo / repair paths
+    if (p.spoil && gpos != 0
+            && (p.spoil == 2 || (lane == 0 && (p.spoil == 1 || (p.spoil == 3 && t0 / kTile % 7 == 0)))))
+        y = y > 16000 ? y - 999 : y + 999; // tests: force the redo / repair paths
     int const y_b = y, xp_b = xp;
     int y_end = y, cmin = 32767, cmax = 0;
     // verify / redo loop: a lane's state at its chunk boundary must be what its left neighbour ended with; the
@@ -365,6 +388,19 @@ __global__ void __launch_bounds__(kFrontWarps * 32, kFrontCtasPerSm) k_front(Fro
     ci.cmin = (int16_t)(nv > 0 ? cmin : 32767);
     ci.cmax = (int16_t)(nv > 0 ? cmax : 0);
     p.chunks[(p.am_offsets[s] + gpos) / C] = ci;
+    int const tmin = __reduce_min_sync(0xffffffffu, nv > 0 ? cmin : 32767);
+    int const tmax = __reduce_max_sync(0xffffffffu, nv > 0 ? cmax : -32768);
+    int const last = __shfl_sync(0xffffffffu, y_end, (nv_tile - 1) / C);
+    if (lane == 0) {
+        TileInfo ti;
+        ti.tmin = (int16_t)tmin;
+        ti.tmax = (int16_t)tmax;
+        ti.first = *reinterpret_cast<int16_t const *>(stage + St::out_at(0));
+        ti.last = (int16_t)last;
+        ti.xsum = x0 + xp_b; // lane 0's x[-1]: narrowed above when the tile starts a block
+        ti.pad = 0;
+        p.tile_info[(p.am_offsets[s] + t0) / kTile] = ti;
+    }
 }
 
 } // namespace r433b

@@ -110,7 +110,7 @@ class Timing(C.Structure):
     _fields_ = [("h2d_ms", C.c_float), ("detect_ms", C.c_float), ("slice_ms", C.c_float), ("d2h_ms", C.c_float),
                 ("total_ms", C.c_float), ("detect_launches", C.c_uint32), ("slice_launches", C.c_uint32),
                 ("front_ms", C.c_float), ("front_launches", C.c_uint32), ("front_redone", C.c_uint32),
-                ("front_repairs", C.c_uint32)]
+                ("front_repairs", C.c_uint32), ("idle_skipped", C.c_uint32), ("idle_rewalks", C.c_uint32)]
 
 
 class PulseData(C.Structure):

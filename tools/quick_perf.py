@@ -65,7 +65,7 @@ for it in range(a.iters):
     tm = ctx.timing()
     c = ctx.counts()
     ms = tm["detect_ms"] + tm["slice_ms"]
-    print(f"iter {it}: front {tm['front_ms']:.2f} redone {tm['front_redone']} repaired {tm['front_repairs']} wall {_wall:.2f} ms ({c['samples'] / _wall / 1e3:.0f} MS/s) detect {tm['detect_ms']:.2f} ms  slice {tm['slice_ms']:.2f} ms  launches {tm['detect_launches']}+{tm['slice_launches']}  "
+    print(f"iter {it}: front {tm['front_ms']:.2f} redone {tm['front_redone']} repaired {tm['front_repairs']} idle skipped {tm['idle_skipped']} rewalks {tm['idle_rewalks']} wall {_wall:.2f} ms ({c['samples'] / _wall / 1e3:.0f} MS/s) detect {tm['detect_ms']:.2f} ms  slice {tm['slice_ms']:.2f} ms  launches {tm['detect_launches']}+{tm['slice_launches']}  "
           f"packages {c['packages']} events {c['events']} event_bytes {c['event_bytes']}  "
           f"-> {c['samples'] / ms / 1e3:.1f} MS/s  detect-only {c['samples'] / tm['detect_ms'] / 1e3:.1f} MS/s "
           f"({c['samples'] * fmt / tm['detect_ms'] / 1e6:.1f} GB/s)")
