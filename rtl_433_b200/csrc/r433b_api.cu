@@ -527,7 +527,6 @@ int r433b_process(r433b_ctx *ctx, r433b_batch const *b)
     dp.am = (int16_t *)ctx->d_am.p;
     dp.chunks = (ChunkInfo const *)ctx->d_chunks.p;
     dp.tile_info = (TileInfo const *)ctx->d_tiles.p;
-    dp.want_stages = b->want_stages ? 1 : 0;
     dp.fm_out = b->want_stages ? (int16_t *)ctx->d_fm.p : nullptr;
 
     uint64_t max_samples = 0;
@@ -596,6 +595,7 @@ int r433b_process(r433b_ctx *ctx, r433b_batch const *b)
         G = (total_bytes >= (256ull << 20) && stride >= (1u << 20)) ? (int)std::min<uint64_t>(r433b_ctx::kMaxGroups, stride / min_slice) : 1;
     }
     if (b->data_on_device && ctx->pipeline_groups == 0) G = 1; // device input: slices only when asked for
+    // stage arrays: k_detect's stage pass makes FM of whole streams, so that batch must be one launch
     if (b->want_stages || !n_devs || !uniform || cf32) G = 1;
     uint64_t slice_samples = 0;
     if (G > 1) {

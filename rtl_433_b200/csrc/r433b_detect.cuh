@@ -20,11 +20,12 @@
 //     pulse of a package, and by the carrier estimate `fsk_f1_est`, which is reported when a package ends.
 //     Neither needs FM for every sample:
 //       * FM WINDOWS of 256 samples are made on demand (discriminator lane-parallel from the IQ bytes,
-//         low-pass by sub-chunks with the same start-from-a-guess / verify / redo scheme).  The filter state
-//         in front of a window that does not continue the previous one is rebuilt RIGOROUSLY: both ends of
-//         the whole state range are pushed through the samples in front of the window until they meet
-//         (monotone filter: the host proves a1, b0 >= 0, a1 + 2 b0 <= unity; otherwise FM is made for
-//         every window of every tile).
+//         low-pass by sub-chunks with the same start-from-a-guess / verify / redo scheme).  A window that does
+//         not continue the previous one closely gets its filter state rebuilt RIGOROUSLY when the filter is
+//         monotone (the host proves a1, b0 >= 0, a1 + 2 b0 <= unity): both ends of the whole state range are
+//         pushed through the samples in front of the window until they meet.  Otherwise the walk reads FM
+//         in order only, and the windows in between are made from the last exact state.  The stage dump
+//         (FM of every sample) is a pass of its own after the walk.
 //       * the carrier estimate g' = g + f/64 - g/64 is DEFERRED after the first pulse: the walk only logs
 //         which samples update it.  When the package ends, g is evaluated over the newest ~1000 logged
 //         samples from both ends of its range; the recurrence forgets its start at 63/64 per sample, the two
@@ -41,9 +42,6 @@
 #include "r433b_core.cuh"
 #include "r433b_front.cuh"
 
-#ifndef R4_REC
-#define R4_REC 2 // recurrence loop of burst_run: 0 always clamped, 1 clamp decided per 8 steps, 2 per stretch
-#endif
 namespace r433b {
 
 constexpr int kTrainInts = 4 * kMaxPulses; // per-stream scratch: ook pulse/gap, fsk pulse/gap
@@ -56,7 +54,6 @@ constexpr int kFmWin = 256;                // FM window
 constexpr int kFmSub = kFmWin / 32;        // samples per lane of a window
 constexpr int kFmPadded = kFmWin + kFmWin / kFmSub; // padded index space: i + i / kFmSub
 constexpr int kWarmFm = 48;                // warm-up samples of the FM trajectories
-constexpr int kFmWindowsPerTile = kTile / kFmWin;
 constexpr unsigned kLogCap = 1024;         // deferred carrier-estimate log: entries per stream
 #ifndef R4_F1_TAIL
 #define R4_F1_TAIL 1024
@@ -69,11 +66,17 @@ struct FmJob {
     uint8_t const *src;        // the stream
     unsigned long long N;      // its length in samples
     long long a1, b0;
-    int16_t *fm_out;           // stage dump (absolute index = stream base + sample) or nullptr
+    int16_t *fm_out;           // stage dump (indexed by sample) or nullptr; the walk's is always nullptr
     unsigned flip;
     int fm_on;                 // 0: "FM" is the raw envelope (buf.fm aliases buf.temp when nothing asks for FM)
     int use_mag;
     int monotone;              // the state rebuild by range collapse is valid
+};
+
+// The exact FM filter state (y, xf) after sample pos - 1
+struct FmState {
+    unsigned long long pos;
+    int y, xf;
 };
 
 // Warp-uniform state of the walk.  It lives in shared memory BETWEEN the phases of the walk (idle_run, burst_run,
@@ -97,7 +100,7 @@ struct WalkConst {
     Trains tr;
     unsigned *log;
     Levels lv;
-    int per_ms, fpdm, lazy_fm, defer_f1;
+    int per_ms, fpdm, defer_f1;
     unsigned stream, block_samples;
     r433b_package *pkgs;
     int *pulse_pool, *gap_pool;
@@ -114,13 +117,9 @@ struct alignas(16) WarpSmem {
     int q[32];                   // chain operands of one 32-sample step
     int cmin[32], cmax[32];      // per lane chunk: bounds of its AM values
     // FM bookkeeping (warp-uniform; written by lane 0)
-    unsigned long long fm_pos;   // (fm_y, fm_xf) is the exact filter state after sample fm_pos - 1
-    int fm_y, fm_xf;
+    FmState fm_state;
     unsigned long long win0;     // the window holds FM of [win0, win0 + win_n)
     int win_n;
-    int tile_state_y[kFmWindowsPerTile], tile_state_xf[kFmWindowsPerTile]; // eager mode: state in front of each window
-    unsigned long long tile_end_pos; // eager mode: the contiguous filter state at the end of the tile pass
-    int tile_end_y, tile_end_xf;
     WalkState ws;
     WalkConst wc;
 };
@@ -129,8 +128,7 @@ struct alignas(16) WarpSmem {
 struct StreamState {
     DetState d;
     int y_am;
-    unsigned long long fm_pos;
-    int fm_y, fm_xf;
+    FmState fm_state;
     unsigned log_n, last_start, last_count;
     unsigned seq;
     int flushed;
@@ -147,7 +145,6 @@ struct DetectParams {
     int first_chunk;                   // start from reset_sdr_flow() state instead of the saved one
     struct StreamState *state;         // per-stream carried state between launches of one batch
     int use_mag, enable_fm, fpdm;
-    int want_stages; // the FM stage array is wanted for every sample (fm_out)
     unsigned flip; // XOR mask applied to every loaded word: 0x80808080 turns cs8 into cu8
     unsigned rate, block_samples;
     Levels lv;
@@ -163,7 +160,7 @@ struct DetectParams {
     int16_t *am;               // k_front's output (repaired in place where a tile did not fit its predecessor)
     ChunkInfo const *chunks;   // bounds of every 64-sample chunk of `am`
     TileInfo const *tile_info; // summary of every tile of `am` (as k_front made it: never updated by a repair)
-    int16_t *fm_out;           // optional stage dump, indexed by offsets[s]/SS + n
+    int16_t *fm_out;           // optional stage dump, indexed by offsets[s]/SS + n (one launch over whole streams)
 };
 
 struct WarpCtx {
@@ -265,13 +262,13 @@ __device__ R4_NOINLINE void disc_fill(FmJob const &jb, WarpSmem &sm, unsigned lo
 // The exact FM filter state in front of sample `pos` (after sample pos - 1), without knowing anything
 // before: both ends of the state range go through the K samples in front of pos; when they meet, the value
 // is independent of everything earlier.  K grows until they meet or the walk starts at a known state
-// (the stream start, or sm.fm_pos).  Monotone filters only.  Leaves the state in sm.fm_pos / fm_y / fm_xf.
+// (the stream start, or sm.fm_state.pos).  Monotone filters only.  Leaves the state in sm.fm_state.
 template <int SS>
 __device__ R4_NOINLINE void fm_cold(FmJob const &jb, WarpSmem &sm, unsigned long long pos)
 {
     constexpr int SPL = 16 / SS;
     int const lane = threadIdx.x & 31;
-    unsigned long long const known = sm.fm_pos; // state known here (always <= pos when used)
+    unsigned long long const known = sm.fm_state.pos; // state known here (always <= pos when used)
     for (unsigned long long K = 64;; K *= 4) {
         unsigned long long a = pos > K ? (pos - K) / SPL * SPL : 0;
         bool exact_start = a == 0;
@@ -281,8 +278,8 @@ __device__ R4_NOINLINE void fm_cold(FmJob const &jb, WarpSmem &sm, unsigned long
             exact_start = true;
         }
         if (exact_start) {
-            lo = hi = a == known ? sm.fm_y : 0;
-            fp = a == known ? sm.fm_xf : 0;
+            lo = hi = a == known ? sm.fm_state.y : 0;
+            fp = a == known ? sm.fm_state.xf : 0;
         } else {
             lo = SS == 2 ? -32768 : (int)0x80000000;
             hi = SS == 2 ? 32767 : 0x7fffffff;
@@ -310,9 +307,7 @@ __device__ R4_NOINLINE void fm_cold(FmJob const &jb, WarpSmem &sm, unsigned long
         }
         if (lo == hi) {
             if (lane == 0) {
-                sm.fm_pos = pos;
-                sm.fm_y = lo;
-                sm.fm_xf = fp;
+                sm.fm_state = FmState{pos, lo, fp};
                 sm.win_n = 0;
             }
             __syncwarp();
@@ -322,8 +317,8 @@ __device__ R4_NOINLINE void fm_cold(FmJob const &jb, WarpSmem &sm, unsigned long
     }
 }
 
-// FM of the window [w0, w0 + n) (n <= kFmWin, w0 a multiple of SPL) from the exact state in sm.fm_* which
-// must be the one in front of w0.  Advances sm.fm_pos to w0 + n.
+// FM of the window [w0, w0 + n) (n <= kFmWin, w0 a multiple of SPL) from the exact state in sm.fm_state which
+// must be the one in front of w0.  Advances sm.fm_state to w0 + n.
 template <int SS>
 __device__ R4_NOINLINE void fm_window(FmJob const &jb, WarpSmem &sm, unsigned long long w0, int n)
 {
@@ -338,11 +333,11 @@ __device__ R4_NOINLINE void fm_window(FmJob const &jb, WarpSmem &sm, unsigned lo
         int y, fp;
         if (exact) {
             start = 0;
-            y = sm.fm_y;
-            fp = sm.fm_xf;
+            y = sm.fm_state.y;
+            fp = sm.fm_state.xf;
         } else {
             fp = (int)sm.xf[fm_pidx(start - 1)];
-            y = SS == 2 ? fp : fp; // the low-pass has unit gain: its state is near its input
+            y = fp; // the low-pass has unit gain: its state is near its input
         }
         if (nv > 0) {
 #pragma unroll 4
@@ -383,12 +378,12 @@ __device__ R4_NOINLINE void fm_window(FmJob const &jb, WarpSmem &sm, unsigned lo
         int ye = __shfl_sync(0xffffffffu, y_end, last);
         int fe = __shfl_sync(0xffffffffu, fp, last);
         if (lane == 0) {
-            sm.fm_y = ye;
-            sm.fm_xf = fe;
+            sm.fm_state.y = ye;
+            sm.fm_state.xf = fe;
         }
     }
     if (lane == 0) {
-        sm.fm_pos = w0 + n;
+        sm.fm_state.pos = w0 + n;
         sm.win0 = w0;
         sm.win_n = n;
     }
@@ -398,54 +393,38 @@ __device__ R4_NOINLINE void fm_window(FmJob const &jb, WarpSmem &sm, unsigned lo
     }
 }
 
-// Make the window that holds sample `pos` current (lazy mode): continue the previous window when it ends
-// close in front, rebuild the state otherwise.
+// Make a window that holds sample `pos` current: continue the previous window when it ends close in front,
+// rebuild the state otherwise (monotone filter).  A filter that is not monotone cannot be rebuilt, but then the
+// carrier estimate is not deferred (defer_f1 == 0): f1_evaluate never runs and the walk asks for FM at increasing
+// positions only, so the state is never behind w0 and the windows in between are made from it.
+// `pos` lies in or in front of the tile being walked; the window ends with that tile (a time slice may end there).
 template <int SS>
-__device__ R4_NOINLINE void fm_demand(FmJob const &jb, WarpSmem &sm, unsigned long long pos, unsigned long long limit)
+__device__ R4_NOINLINE void fm_demand(FmJob const &jb, WarpSmem &sm, unsigned long long pos)
 {
     constexpr int SPL = 16 / SS;
+    unsigned long long const limit = sm.ws.t0 + (unsigned long long)sm.ws.nv_tile;
     unsigned long long w0 = pos / SPL * SPL;
     if (jb.fm_on) {
-        unsigned long long const have = sm.fm_pos;
-        if (have > w0 || w0 - have > 2 * kFmWin) {
+        unsigned long long const have = sm.fm_state.pos;
+        if (jb.monotone && (have > w0 || w0 - have > 2 * kFmWin)) {
             fm_cold<SS>(jb, sm, w0);
         } else {
-            while (sm.fm_pos + kFmWin <= w0) fm_window<SS>(jb, sm, sm.fm_pos, kFmWin); // walk up to it
-            w0 = sm.fm_pos;
+#ifdef R433B_SIMT_EMU
+            assert(have <= w0);
+#endif
+            while (sm.fm_state.pos + kFmWin <= w0) fm_window<SS>(jb, sm, sm.fm_state.pos, kFmWin); // walk up to it
+            w0 = sm.fm_state.pos;
         }
     }
     unsigned long long end = w0 + kFmWin < limit ? w0 + kFmWin : limit;
     fm_window<SS>(jb, sm, w0, (int)(end - w0));
 }
 
-// The window for the detector walk at tile [t0, t0 + nv_tile): on demand (lazy), or re-made from the start
-// states the tile pass kept (eager mode: windows are aligned, the end-of-tile state is put back afterwards).
+// FM of sample `pos` is in sm.fm after this: the current window holds it, or one is made on demand
 template <int SS>
-__device__ R4_NOINLINE void fm_for_walk(FmJob const &jb, WarpSmem &sm, unsigned long long pos, unsigned long long t0,
-        int nv_tile, bool lazy)
+__device__ __forceinline__ void fm_cover(FmJob const &jb, WarpSmem &sm, unsigned long long pos)
 {
-    int const lane = threadIdx.x & 31;
-    if (lazy) {
-        fm_demand<SS>(jb, sm, pos, t0 + (unsigned long long)nv_tile);
-        return;
-    }
-    int const w = (int)(pos - t0) / kFmWin;
-    if (lane == 0) {
-        sm.fm_y = sm.tile_state_y[w];
-        sm.fm_xf = sm.tile_state_xf[w];
-        sm.fm_pos = t0 + (unsigned long long)w * kFmWin;
-    }
-    __syncwarp();
-    FmJob quiet = jb;
-    quiet.fm_out = nullptr;
-    int const cnt = nv_tile - w * kFmWin < kFmWin ? nv_tile - w * kFmWin : kFmWin;
-    fm_window<SS>(quiet, sm, t0 + (unsigned long long)w * kFmWin, cnt);
-    if (lane == 0) {
-        sm.fm_pos = sm.tile_end_pos;
-        sm.fm_y = sm.tile_end_y;
-        sm.fm_xf = sm.tile_end_xf;
-    }
-    __syncwarp();
+    if (!(sm.win_n > 0 && pos >= sm.win0 && pos < sm.win0 + (unsigned long long)sm.win_n)) fm_demand<SS>(jb, sm, pos);
 }
 
 // ---------------------------------------------------- deferred carrier estimate ---------
@@ -495,8 +474,7 @@ __device__ R4_NOINLINE int f1_evaluate(FmJob const &jb, WarpSmem &sm, unsigned c
             entry(j, st, cnt);
             unsigned long long pos = start_abs + st;
             while (cnt) {
-                if (!(sm.win_n > 0 && pos >= sm.win0 && pos < sm.win0 + (unsigned long long)sm.win_n))
-                    fm_demand<SS>(jb, sm, pos, jb.N);
+                fm_cover<SS>(jb, sm, pos);
                 unsigned long long wend = sm.win0 + (unsigned long long)sm.win_n;
                 unsigned take = wend - pos < cnt ? (unsigned)(wend - pos) : cnt;
                 int const i0 = (int)(pos - sm.win0);
@@ -592,18 +570,6 @@ __device__ __forceinline__ bool log_add(LogRegs &L, unsigned *log, unsigned rel,
     return true;
 }
 
-// eager FM mode: put the contiguous end-of-tile filter state back after windows were (re-)made out of order
-__device__ __forceinline__ void restore_tile_end(WarpSmem &sm)
-{
-    __syncwarp();
-    if ((threadIdx.x & 31) == 0 && !sm.wc.lazy_fm) {
-        sm.fm_pos = sm.tile_end_pos;
-        sm.fm_y = sm.tile_end_y;
-        sm.fm_xf = sm.tile_end_xf;
-    }
-    __syncwarp();
-}
-
 // everything logged so far into the exact value ws.d.ook_f1 (state in shared memory)
 template <int SS>
 __device__ R4_NOINLINE void walk_f1_fold(WarpSmem &sm)
@@ -611,7 +577,7 @@ __device__ R4_NOINLINE void walk_f1_fold(WarpSmem &sm)
     __syncwarp();
     int const g = f1_evaluate<SS>(sm.wc.jb, sm, sm.wc.log, sm.ws.d.start_abs, sm.ws.d.ook_f1, sm.ws.log_n, sm.ws.log_start,
             sm.ws.log_count);
-    restore_tile_end(sm);
+    // the log is not empty, so f1_evaluate synchronised the warp after every lane had read its arguments
     if ((threadIdx.x & 31) == 0) {
         sm.ws.d.ook_f1 = g;
         sm.ws.log_n = 0;
@@ -705,6 +671,13 @@ struct IdleRegs {
     int low, high, lead_in;
 };
 
+// `high` as IDLE derives it from `low` (src/pulse_detect.c:331-332)
+__device__ __forceinline__ int derived_high(int low, Levels const &lv)
+{
+    int const h = lv.ratio * low;
+    return h < lv.min_high ? lv.min_high : h;
+}
+
 // IDLE over a long stretch of the tile in sm.am from sample n on, lane-parallel: see the comment in the file header
 // and below.  While |am - low| < 1024 the tracker is low += (am > low) ? +1 : -1, so low keeps the parity of
 // (low0 + samples seen) and two trajectories of equal parity never cross and merge once the data passes between
@@ -739,9 +712,7 @@ __device__ __forceinline__ int idle_tile(WarpSmem const &sm, IdleRegs &d, int n,
     }
     int Lmin = lo0 < pmin - 1 ? lo0 : pmin - 1;
     int Lmax = hi0 > pmax ? hi0 : pmax;
-    int hmin = lv.ratio * Lmin;
-    if (hmin < lv.min_high) hmin = lv.min_high;
-    Thresholds th = det_thresholds(Lmin, hmin, lv);
+    Thresholds th = det_thresholds(Lmin, derived_high(Lmin, lv), lv);
     bool const armed = d.lead_in + (nv_tile - n) > kLeadIn;
     bool ok = in_region && !(armed && cmax > th.up) && (pmax - Lmin < 1024) && (Lmax - pmin < 1024);
     unsigned bad = ~__ballot_sync(0xffffffffu, ok) & (0xffffffffu << c0);
@@ -810,8 +781,7 @@ __device__ __forceinline__ int idle_tile(WarpSmem const &sm, IdleRegs &d, int n,
     if (!done) return 0;
     int const len = (e * C < nv_tile ? e * C : nv_tile) - n;
     d.low = result;
-    int hh = lv.ratio * d.low;
-    d.high = hh < lv.min_high ? lv.min_high : hh;
+    d.high = derived_high(d.low, lv);
     int li = d.lead_in + len;
     d.lead_in = li > kLeadIn + 1 ? kLeadIn + 1 : li;
     return len;
@@ -837,9 +807,7 @@ __device__ R4_NOINLINE int idle_run(WarpSmem &sm, int n)
         int cnt = nv_tile - n < 32 ? nv_tile - n : 32;
         int a = lane < cnt ? am_at(n + lane) : -32768;
         int lmin = d.low - cnt;
-        int hmin = lv.ratio * lmin;
-        if (hmin < lv.min_high) hmin = lv.min_high;
-        Thresholds th = det_thresholds(lmin, hmin, lv); // lowest trigger level reachable in this chunk
+        Thresholds th = det_thresholds(lmin, derived_high(lmin, lv), lv); // lowest trigger level reachable in this chunk
         bool armed = d.lead_in + cnt - 1 > kLeadIn;
         bool stop = lane < cnt && ((armed && a > th.up) || (a - lmin >= 1024) || (d.low + cnt - a >= 1024));
         unsigned m = __ballot_sync(0xffffffffu, stop);
@@ -865,8 +833,7 @@ __device__ R4_NOINLINE int idle_run(WarpSmem &sm, int n)
         for (; j < cnt; ++j)
             if (sm.q[j] > q) q += 2;
         d.low = q - cnt;
-        int hh = lv.ratio * d.low;
-        d.high = hh < lv.min_high ? lv.min_high : hh;
+        d.high = derived_high(d.low, lv);
         int li = d.lead_in + cnt;
         d.lead_in = li > kLeadIn + 1 ? kLeadIn + 1 : li;
         return cnt;
@@ -874,9 +841,7 @@ __device__ R4_NOINLINE int idle_run(WarpSmem &sm, int n)
 
 
     while (n < nv_tile) {
-        int hs = lv.ratio * d.low;
-        if (hs < lv.min_high) hs = lv.min_high;
-        if (d.high != hs) break; // first IDLE sample after a package: not yet re-derived
+        if (d.high != derived_high(d.low, lv)) break; // first IDLE sample after a package: not yet re-derived
         int adv = idle_tile(sm, d, n, d.low, d.low, lv, nv_tile);
         if (!adv) adv = idle_fast(n);
         if (!adv) break;
@@ -952,11 +917,9 @@ __device__ R4_NOINLINE unsigned long long idle_skip(WarpSmem &sm, int16_t const 
         li = li > kLeadIn + 1 ? kLeadIn + 1 : li;
         int const Lmin = blo < tmin - 1 ? blo : tmin - 1;
         int const Lmax = bhi > tmax ? bhi : tmax;
-        int hmin = lv.ratio * Lmin;
-        if (hmin < lv.min_high) hmin = lv.min_high;
         bool const armed = li + T > kLeadIn;
         bool const ok = inside && iir16_nowrap(yin, a1, b0, ti.xsum) == (int)ti.first && tmax - Lmin < 1024
-                && Lmax - tmin < 1024 && !(armed && tmax > det_thresholds(Lmin, hmin, lv).up);
+                && Lmax - tmin < 1024 && !(armed && tmax > det_thresholds(Lmin, derived_high(Lmin, lv), lv).up);
         unsigned const bad = ~__ballot_sync(0xffffffffu, ok);
         int const e = bad ? __ffs(bad) - 1 : 32; // tiles t .. t + e - 1 are skipped
         if (e == 0) break;
@@ -1019,20 +982,20 @@ __device__ R4_NOINLINE unsigned long long idle_skip(WarpSmem &sm, int16_t const 
     return t0;
 }
 
-    // Everything of a package after its first pulse (and the first real gap), in one loop with the hot
-    // state in registers: src/pulse_detect.c:355-470 without the FSK sub-detector (it is only fed during the
-    // first pulse) and with the carrier estimate deferred (logged).
-    //   PULSE: the high-level estimator (:362-363) is a truncating 64-sample moving average -- inherently
-    //     sequential -- but the pulse only ends on a sample below the threshold its value implies.  One step
-    //     never lifts `high` above max(high, 64 * (am / 64) + 63), so the largest am of 32 samples bounds
-    //     every threshold among them from above: samples not below THAT threshold cannot end the pulse.  The
-    //     recurrence runs over exactly those (operands staged in shared memory, four per load); the first
-    //     sample that might end the pulse is then tested exactly.
-    //   GAP_START / GAP: thresholds are frozen; the next event is the first sample above `up` -- a spurious
-    //     gap if the run is still <= 10 samples, the next pulse otherwise -- or the run length reaching an
-    //     end-of-package limit (:422-470).  32 samples per ballot.
-    // Rare turns (spurious pulse, 1200 pulses) are left to det_step() in the generic step: the loop stops in front of the sample.
-    // Returns the first sample not consumed; a finished package is handed over through pend_type / pend_pos.
+// Everything of a package after its first pulse (and the first real gap), in one loop with the hot
+// state in registers: src/pulse_detect.c:355-470 without the FSK sub-detector (it is only fed during the
+// first pulse) and with the carrier estimate deferred (logged).
+//   PULSE: the high-level estimator (:362-363) is a truncating 64-sample moving average -- inherently
+//     sequential -- but the pulse only ends on a sample below the threshold its value implies.  One step
+//     never lifts `high` above max(high, 64 * (am / 64) + 63), so the largest am of 32 samples bounds
+//     every threshold among them from above: samples not below THAT threshold cannot end the pulse.  The
+//     recurrence runs over exactly those (operands staged in shared memory, four per load); the first
+//     sample that might end the pulse is then tested exactly.
+//   GAP_START / GAP: thresholds are frozen; the next event is the first sample above `up` -- a spurious
+//     gap if the run is still <= 10 samples, the next pulse otherwise -- or the run length reaching an
+//     end-of-package limit (:422-470).  32 samples per ballot.
+// Rare turns (spurious pulse, 1200 pulses) are left to det_step() in the generic step: the loop stops in front of the sample.
+// Returns the first sample not consumed; a finished package is handed over through pend_type / pend_pos.
 __device__ R4_NOINLINE int burst_run(WarpSmem &sm, int n)
 {
     int const lane = threadIdx.x & 31;
@@ -1054,28 +1017,28 @@ __device__ R4_NOINLINE int burst_run(WarpSmem &sm, int n)
     int pend_type = 0;
     unsigned long long pend_pos = 0;
     auto am_at = [&](int i) -> int { return am_tile_at(am16, i); };
-        int st = d.st, run = d.run, h = d.high;
-        int const low = d.low, minh = lv.min_high;
+    int st = d.st, run = d.run, h = d.high;
+    int const low = d.low, minh = lv.min_high;
 #pragma unroll 1
-        while (n < nv_tile) {
-            if (st == kPulse) {
-                if (d.ook_n == 0) break; // a first pulse feeds the FSK sub-detector: not here
-                unsigned const rel = (unsigned)(t0 + (unsigned long long)n - d.start_abs);
-                // a full log is folded by the generic step first (nothing has been touched yet)
-                if (L.count && L.start + L.count != rel && L.n == kLogCap) break;
-                int cnt = nv_tile - n < 32 ? nv_tile - n : 32;
-                int const a = lane < cnt ? am_at(n + lane) : 32767;
-                int const aq = a >> 6; // am >= 0
-                int const top = __reduce_max_sync(0xffffffffu, lane < cnt ? aq : 0); // one REDUX each
-                    int hmax = 64 * top + 63;
-                hmax = h > hmax ? h : hmax;
-                unsigned const m = __ballot_sync(0xffffffffu, lane < cnt && a < det_thresholds(low, hmax, lv).down);
-                if (m) cnt = __ffs(m) - 1;
-                if (cnt) {
-                    __syncwarp();
-                    sm.q[lane] = aq;
-                    __syncwarp();
-                    // h >= min_high >= 0 here, so h / 64 == h >> 6.  Eight steps per trip, the loops kept rolled: seven
+    while (n < nv_tile) {
+        if (st == kPulse) {
+            if (d.ook_n == 0) break; // a first pulse feeds the FSK sub-detector: not here
+            unsigned const rel = (unsigned)(t0 + (unsigned long long)n - d.start_abs);
+            // a full log is folded by the generic step first (nothing has been touched yet)
+            if (L.count && L.start + L.count != rel && L.n == kLogCap) break;
+            int cnt = nv_tile - n < 32 ? nv_tile - n : 32;
+            int const a = lane < cnt ? am_at(n + lane) : 32767;
+            int const aq = a >> 6; // am >= 0
+            int const top = __reduce_max_sync(0xffffffffu, lane < cnt ? aq : 0); // one REDUX each
+            int hmax = 64 * top + 63;
+            hmax = h > hmax ? h : hmax;
+            unsigned const m = __ballot_sync(0xffffffffu, lane < cnt && a < det_thresholds(low, hmax, lv).down);
+            if (m) cnt = __ffs(m) - 1;
+            if (cnt) {
+                __syncwarp();
+                sm.q[lane] = aq;
+                __syncwarp();
+                // h >= min_high >= 0 here, so h / 64 == h >> 6.  Eight steps per trip, the loops kept rolled: seven
                 // warps per scheduler share an instruction cache of a few hundred instructions.
                 // q >= 0, so one step takes at most h >> 6 off, and less from a lower h: after k steps h is still
                 // >= h0 - k (h0 >> 6).  If that stays >= min_high over the whole stretch the clamp of :363 cannot act
@@ -1084,7 +1047,6 @@ __device__ R4_NOINLINE int burst_run(WarpSmem &sm, int n)
                 int trips = cnt >> 3;
 #define R4_STEP(q) h += (q) - (int)((unsigned)h >> 6)
 #define R4_STEP_CLAMPED(q) h = max(h + (q) - (int)((unsigned)h >> 6), minh)
-#if R4_REC == 2
                 if (h - cnt * (int)((unsigned)h >> 6) >= minh) {
 #pragma unroll 1
                     for (; trips > 0; --trips, qp += 2) {
@@ -1100,117 +1062,99 @@ __device__ R4_NOINLINE int burst_run(WarpSmem &sm, int n)
                         R4_STEP_CLAMPED(c.x); R4_STEP_CLAMPED(c.y); R4_STEP_CLAMPED(c.z); R4_STEP_CLAMPED(c.w);
                     }
                 }
-#elif R4_REC == 1
-#pragma unroll 1
-                for (; trips > 0; --trips, qp += 2) {
-                    int4 const b = qp[0], c = qp[1];
-                    if (h - 8 * (int)((unsigned)h >> 6) >= minh) {
-                        R4_STEP(b.x); R4_STEP(b.y); R4_STEP(b.z); R4_STEP(b.w);
-                        R4_STEP(c.x); R4_STEP(c.y); R4_STEP(c.z); R4_STEP(c.w);
-                    } else {
-                        R4_STEP_CLAMPED(b.x); R4_STEP_CLAMPED(b.y); R4_STEP_CLAMPED(b.z); R4_STEP_CLAMPED(b.w);
-                        R4_STEP_CLAMPED(c.x); R4_STEP_CLAMPED(c.y); R4_STEP_CLAMPED(c.z); R4_STEP_CLAMPED(c.w);
-                    }
-                }
-#else
-#pragma unroll 1
-                for (; trips > 0; --trips, qp += 2) {
-                    int4 const b = qp[0], c = qp[1];
-                    R4_STEP_CLAMPED(b.x); R4_STEP_CLAMPED(b.y); R4_STEP_CLAMPED(b.z); R4_STEP_CLAMPED(b.w);
-                    R4_STEP_CLAMPED(c.x); R4_STEP_CLAMPED(c.y); R4_STEP_CLAMPED(c.z); R4_STEP_CLAMPED(c.w);
-                }
-#endif
+#undef R4_STEP
+#undef R4_STEP_CLAMPED
                 {
                     int const *qs = reinterpret_cast<int const *>(qp);
 #pragma unroll 1
                     for (int r = cnt & 7; r > 0; --r, ++qs) h = max(h + *qs - (int)((unsigned)h >> 6), minh);
                 }
                 log_add(L, log, rel, (unsigned)cnt, lane);
-                    run += cnt;
-                    n += cnt;
-                }
-                if (m) { // the sample at n might end the pulse: the exact test of :355
-                    int const aj = __shfl_sync(0xffffffffu, a, cnt);
-                    if (aj < det_thresholds(low, h, lv).down) {
-                        if (run + 1 < kMinPulseSamples) break; // spurious pulse (:341-350)
-                        run += 1;
-                        put(tr.ook_pulse, d.ook_hw, d.ook_n, run);
-                        d.last_pulse = run;
-                        if (run > d.longest) d.longest = run;
-                        run = 0;
-                        st = kGapStart;
-                    } else {
-                        h += (aj >> 6) - (int)((unsigned)h >> 6);
-                        h = h < minh ? minh : h;
-                        log_add(L, log, (unsigned)(t0 + (unsigned long long)n - d.start_abs), 1u, lane);
-                        run += 1;
-                    }
-                    n += 1;
-                }
-                continue;
+                run += cnt;
+                n += cnt;
             }
-            // GAP_START (run <= 9 so far) or GAP
-            int const cnt = nv_tile - n;
-            int const up = det_thresholds(low, h, lv).up;
-            // min(max(10 * longest, 10 * per_ms), 100 * per_ms) in 32 bits: a pulse of 10 * per_ms samples or more makes
-            // the first limit reach the second, so `longest` can be capped there (per_ms <= 2^31 / 1000: no overflow)
-            int const lim_b = 100 * per_ms;
-            int const lcap = d.longest < 10 * per_ms ? d.longest : 10 * per_ms;
-            int const lim_a = lcap > per_ms ? 10 * lcap : 10 * per_ms;
-            int const rstar = (lim_a < lim_b ? lim_a : lim_b) + 1; // first run length that ends the package
-            int je = rstar - run - 1;                               // ... reached at this sample of the scan
-            // the limits are only looked at in GAP, i.e. from the sample after the one that brought the run to 10
-            int const first_gap = st == kGapStart ? kMinPulseSamples - run : 0;
-            if (je < first_gap) je = first_gap;
-            int const horizon = je < cnt ? je + 1 : cnt; // samples that matter
-            int ja = 0x7fffffff;
+            if (m) { // the sample at n might end the pulse: the exact test of :355
+                int const aj = __shfl_sync(0xffffffffu, a, cnt);
+                if (aj < det_thresholds(low, h, lv).down) {
+                    if (run + 1 < kMinPulseSamples) break; // spurious pulse (:341-350)
+                    run += 1;
+                    put(tr.ook_pulse, d.ook_hw, d.ook_n, run);
+                    d.last_pulse = run;
+                    if (run > d.longest) d.longest = run;
+                    run = 0;
+                    st = kGapStart;
+                } else {
+                    h += (aj >> 6) - (int)((unsigned)h >> 6);
+                    h = h < minh ? minh : h;
+                    log_add(L, log, (unsigned)(t0 + (unsigned long long)n - d.start_abs), 1u, lane);
+                    run += 1;
+                }
+                n += 1;
+            }
+            continue;
+        }
+        // GAP_START (run <= 9 so far) or GAP
+        int const cnt = nv_tile - n;
+        int const up = det_thresholds(low, h, lv).up;
+        // min(max(10 * longest, 10 * per_ms), 100 * per_ms) in 32 bits: a pulse of 10 * per_ms samples or more makes
+        // the first limit reach the second, so `longest` can be capped there (per_ms <= 2^31 / 1000: no overflow)
+        int const lim_b = 100 * per_ms;
+        int const lcap = d.longest < 10 * per_ms ? d.longest : 10 * per_ms;
+        int const lim_a = lcap > per_ms ? 10 * lcap : 10 * per_ms;
+        int const rstar = (lim_a < lim_b ? lim_a : lim_b) + 1; // first run length that ends the package
+        int je = rstar - run - 1;                               // ... reached at this sample of the scan
+        // the limits are only looked at in GAP, i.e. from the sample after the one that brought the run to 10
+        int const first_gap = st == kGapStart ? kMinPulseSamples - run : 0;
+        if (je < first_gap) je = first_gap;
+        int const horizon = je < cnt ? je + 1 : cnt; // samples that matter
+        int ja = 0x7fffffff;
 #pragma unroll 1
-            for (int base = 0; base < horizon; base += 32) {
-                int const a = base + lane < cnt ? am_at(n + base + lane) : -32768;
-                unsigned const m = __ballot_sync(0xffffffffu, a > up);
-                if (m) {
-                    ja = base + __ffs(m) - 1;
-                    break;
-                }
+        for (int base = 0; base < horizon; base += 32) {
+            int const a = base + lane < cnt ? am_at(n + base + lane) : -32768;
+            unsigned const m = __ballot_sync(0xffffffffu, a > up);
+            if (m) {
+                ja = base + __ffs(m) - 1;
+                break;
             }
-            if (ja < cnt && ja <= je) {
-                if (st == kGapStart && run + ja + 1 <= kMinPulseSamples) { // spurious gap (:379-385)
-                    run += ja + 1 + d.last_pulse;
-                    st = kPulse;
-                    n += ja + 1;
-                    continue;
-                }
-                if (d.ook_n + 1 >= (unsigned)kMaxPulses) { // the 1200th pulse ends the package (:429-441): det_step()
-                    run += ja;
-                    n += ja;
-                    st = run >= kMinPulseSamples ? kGap : kGapStart;
-                    break;
-                }
-                run += ja + 1; // a new pulse starts (:422-428)
-                put(tr.ook_gap, d.ook_hw, d.ook_n, run);
-                d.ook_n += 1;
-                run = 0;
+        }
+        if (ja < cnt && ja <= je) {
+            if (st == kGapStart && run + ja + 1 <= kMinPulseSamples) { // spurious gap (:379-385)
+                run += ja + 1 + d.last_pulse;
                 st = kPulse;
                 n += ja + 1;
                 continue;
             }
-            if (je < cnt) { // end of package by gap length (:443-469)
-                run += je + 1;
-                put(tr.ook_gap, d.ook_hw, d.ook_n, run);
-                d.ook_n += 1;
-                st = kIdle;
-                pend_type = 1;
-                n += je; // that sample is looked at again in IDLE
-                pend_pos = t0 + (unsigned long long)n;
+            if (d.ook_n + 1 >= (unsigned)kMaxPulses) { // the 1200th pulse ends the package (:429-441): det_step()
+                run += ja;
+                n += ja;
+                st = run >= kMinPulseSamples ? kGap : kGapStart;
                 break;
             }
-            run += cnt;
-            if (run >= kMinPulseSamples) st = kGap;
-            n += cnt;
+            run += ja + 1; // a new pulse starts (:422-428)
+            put(tr.ook_gap, d.ook_hw, d.ook_n, run);
+            d.ook_n += 1;
+            run = 0;
+            st = kPulse;
+            n += ja + 1;
+            continue;
         }
-        d.st = st;
-        d.run = run;
-        d.high = h;
+        if (je < cnt) { // end of package by gap length (:443-469)
+            run += je + 1;
+            put(tr.ook_gap, d.ook_hw, d.ook_n, run);
+            d.ook_n += 1;
+            st = kIdle;
+            pend_type = 1;
+            n += je; // that sample is looked at again in IDLE
+            pend_pos = t0 + (unsigned long long)n;
+            break;
+        }
+        run += cnt;
+        if (run >= kMinPulseSamples) st = kGap;
+        n += cnt;
+    }
+    d.st = st;
+    d.run = run;
+    d.high = h;
 
     __syncwarp();
     if (lane == 0) {
@@ -1256,7 +1200,6 @@ __device__ R4_NOINLINE int first_run(WarpSmem &sm, int n)
     Levels const lv = sm.wc.lv;
     Trains const tr = sm.wc.tr;
     int const fpdm = sm.wc.fpdm, minh = lv.min_high;
-    bool const lazy_fm = sm.wc.lazy_fm != 0;
     int const nv_tile = sm.ws.nv_tile;
     unsigned long long const t0 = sm.ws.t0;
     WarpCtx cx;
@@ -1265,8 +1208,7 @@ __device__ R4_NOINLINE int first_run(WarpSmem &sm, int n)
 #pragma unroll 1
     while (n < nv_tile) {
         unsigned long long const pos = t0 + (unsigned long long)n;
-        if (!(sm.win_n > 0 && pos >= sm.win0 && pos < sm.win0 + (unsigned long long)sm.win_n))
-            fm_for_walk<SS>(sm.wc.jb, sm, pos, t0, nv_tile, lazy_fm);
+        fm_cover<SS>(sm.wc.jb, sm, pos);
         int cnt = nv_tile - n < 32 ? nv_tile - n : 32;
         int const in_win = (int)(sm.win0 + (unsigned long long)sm.win_n - pos);
         cnt = cnt < in_win ? cnt : in_win;
@@ -1333,8 +1275,7 @@ __device__ R4_NOINLINE int generic_step(WarpSmem &sm, int n)
     Trains const tr = sm.wc.tr;
     unsigned *const log = sm.wc.log;
     int const per_ms = sm.wc.per_ms, fpdm = sm.wc.fpdm;
-    bool const defer_f1 = sm.wc.defer_f1 != 0, lazy_fm = sm.wc.lazy_fm != 0;
-    int const nv_tile = sm.ws.nv_tile;
+    bool const defer_f1 = sm.wc.defer_f1 != 0;
     unsigned long long const t0 = sm.ws.t0;
     WarpCtx cx;
     cx.lane = lane;
@@ -1359,18 +1300,12 @@ __device__ R4_NOINLINE int generic_step(WarpSmem &sm, int n)
         L.n = L.count = 0;
         log_add(L, log, rel, cnt, lane);
     };
-    // FM of tile sample i: make the window that holds it current first
-    auto fm_need = [&](int i) {
-        unsigned long long pos = t0 + (unsigned long long)i;
-        if (sm.win_n > 0 && pos >= sm.win0 && pos < sm.win0 + (unsigned long long)sm.win_n) return;
-        fm_for_walk<SS>(sm.wc.jb, sm, pos, t0, nv_tile, lazy_fm);
-    };
     auto fm_at = [&](int i) -> int { return (int)(int16_t)sm.fm[fm_pidx((int)(t0 + (unsigned long long)i - sm.win0))]; };
 
     // inside a first pulse (and its GAP_START) the FSK sub-detector and the undeferred estimate read FM
     bool const first = d.ook_n == 0 && (d.st == kPulse || d.st == kGapStart);
     bool const wants_fm = first || (d.st == kPulse && !defer_f1);
-    if (wants_fm) fm_need(n);
+    if (wants_fm) fm_cover<SS>(sm.wc.jb, sm, t0 + (unsigned long long)n);
     int adv = 0;
     {
         // every lane runs the (warp-uniform) step and writes the same train entries: keep the lanes
@@ -1410,17 +1345,14 @@ __global__ void __launch_bounds__(kDetectWarps * 32, kDetectCtasPerSm) k_detect(
 
     WarpSmem &sm = reinterpret_cast<WarpSmem *>(smem_raw)[warp];
     uint16_t const *am16 = reinterpret_cast<uint16_t const *>(sm.am);
-    bool const fm_on = p.enable_fm != 0;
 
     unsigned long long const byte0 = p.offsets[s];
     unsigned long long const N = (p.lengths ? p.lengths[s] : p.offsets[s + 1] - byte0) / SS;
     uint8_t const *const src = p.data + byte0;
     int16_t *const am_stream = p.am + p.am_offsets[s];
     ChunkInfo const *const chunk_stream = p.chunks + p.am_offsets[s] / kChunk;
-    // FM windows on demand need the rigorous state rebuild (monotone filter); the stage dump wants every sample
-    bool const lazy_fm = !fm_on || (p.wrap_free && !p.want_stages);
-    // the deferred carrier estimate re-makes FM for logged samples later: needs the state rebuild as well
-    bool const defer_f1 = !fm_on || p.wrap_free != 0;
+    // the deferred carrier estimate re-makes FM for logged samples later, out of order: needs the state rebuild
+    bool const defer_f1 = !p.enable_fm || p.wrap_free != 0;
 
     int y_am = 0; // the last AM value of the previous tile: the AM filter state (reset_sdr_flow(): zero)
     int flushed = 0;
@@ -1434,7 +1366,7 @@ __global__ void __launch_bounds__(kDetectWarps * 32, kDetectCtasPerSm) k_detect(
         wc.jb.fm_on = p.enable_fm;
         wc.jb.use_mag = p.use_mag;
         wc.jb.monotone = p.wrap_free;
-        wc.jb.fm_out = p.fm_out ? p.fm_out + byte0 / SS : nullptr;
+        wc.jb.fm_out = nullptr;
         wc.tr.ook_pulse = p.train_scratch + (size_t)s * kTrainInts;
         wc.tr.ook_gap = wc.tr.ook_pulse + kMaxPulses;
         wc.tr.fsk_pulse = wc.tr.ook_gap + kMaxPulses;
@@ -1443,7 +1375,6 @@ __global__ void __launch_bounds__(kDetectWarps * 32, kDetectCtasPerSm) k_detect(
         wc.lv = p.lv;
         wc.per_ms = (int)(p.rate / 1000);
         wc.fpdm = p.fpdm;
-        wc.lazy_fm = lazy_fm;
         wc.defer_f1 = defer_f1;
         wc.stream = s;
         wc.block_samples = p.block_samples;
@@ -1453,8 +1384,7 @@ __global__ void __launch_bounds__(kDetectWarps * 32, kDetectCtasPerSm) k_detect(
         wc.pkg_cap = p.pkg_cap;
         wc.pool_cap = p.pool_cap;
         wc.counters = p.counters;
-        // idle tiles are skipped when nothing but the tracker needs them: no FM made for every tile, no stage dump
-        wc.tiles = lazy_fm && !p.fm_out ? p.tile_info + p.am_offsets[s] / kTile : nullptr;
+        wc.tiles = p.tile_info ? p.tile_info + p.am_offsets[s] / kTile : nullptr;
         WalkState &ws = sm.ws;
         ws.pend_type = 0;
         ws.pend_pos = 0;
@@ -1467,8 +1397,7 @@ __global__ void __launch_bounds__(kDetectWarps * 32, kDetectCtasPerSm) k_detect(
             ws.d.ook_hw = ws.d.fsk_hw = kMaxPulses; // scratch is not assumed to be zero: first package clears it
             ws.log_n = ws.log_start = ws.log_count = 0;
             ws.seq = 0;
-            sm.fm_pos = 0;
-            sm.fm_y = sm.fm_xf = 0;
+            sm.fm_state = FmState{0, 0, 0};
         } else {
             StreamState const &ss = p.state[s];
             ws.d = ss.d;
@@ -1476,9 +1405,7 @@ __global__ void __launch_bounds__(kDetectWarps * 32, kDetectCtasPerSm) k_detect(
             ws.log_n = ss.log_n;
             ws.log_start = ss.last_start;
             ws.log_count = ss.last_count;
-            sm.fm_pos = ss.fm_pos;
-            sm.fm_y = ss.fm_y;
-            sm.fm_xf = ss.fm_xf;
+            sm.fm_state = ss.fm_state;
         }
         sm.win0 = 0;
         sm.win_n = 0;
@@ -1493,9 +1420,7 @@ __global__ void __launch_bounds__(kDetectWarps * 32, kDetectCtasPerSm) k_detect(
 
     for (unsigned long long t0 = p.sample_begin; t0 < p.sample_end && t0 < N; t0 += T) {
         if (sm.wc.tiles && sm.ws.d.st == kIdle && !sm.ws.pend_type && !sm.ws.d.eop_flag && t0 / T >= sm.ws.rewalk_end) {
-            int hs = p.lv.ratio * sm.ws.d.low;
-            if (hs < p.lv.min_high) hs = p.lv.min_high;
-            if (sm.ws.d.high == hs) {
+            if (sm.ws.d.high == derived_high(sm.ws.d.low, p.lv)) {
                 t0 = idle_skip(sm, am_stream, chunk_stream, t0, p.sample_end, y_am, a1, b0);
                 y_am = sm.ws.skip_y;
             }
@@ -1554,24 +1479,6 @@ __global__ void __launch_bounds__(kDetectWarps * 32, kDetectCtasPerSm) k_detect(
             }
         }
         y_am = am_tile_at(am16, nv_tile - 1);
-        // ---- FM for the whole tile when it cannot be made on demand -----------------------------
-        if (!lazy_fm || (!fm_on && p.fm_out)) {
-            for (int w = 0; w * kFmWin < nv_tile; ++w) {
-                if (lane == 0) {
-                    sm.tile_state_y[w] = sm.fm_y;
-                    sm.tile_state_xf[w] = sm.fm_xf;
-                }
-                __syncwarp();
-                int n = nv_tile - w * kFmWin < kFmWin ? nv_tile - w * kFmWin : kFmWin;
-                fm_window<SS>(sm.wc.jb, sm, t0 + (unsigned long long)w * kFmWin, n);
-            }
-            if (lane == 0) {
-                sm.tile_end_pos = sm.fm_pos;
-                sm.tile_end_y = sm.fm_y;
-                sm.tile_end_xf = sm.fm_xf;
-            }
-            __syncwarp();
-        }
 
         // ---- package detector over the tile (warp-uniform), phase by phase ------------------------
         if (t0 % p.block_samples == 0) walk_call_boundary(sm);
@@ -1613,14 +1520,24 @@ __global__ void __launch_bounds__(kDetectWarps * 32, kDetectCtasPerSm) k_detect(
         StreamState &ss = p.state[s];
         ss.d = sm.ws.d;
         ss.y_am = y_am;
-        ss.fm_pos = sm.fm_pos;
-        ss.fm_y = sm.fm_y;
-        ss.fm_xf = sm.fm_xf;
+        ss.fm_state = sm.fm_state;
         ss.log_n = sm.ws.log_n;
         ss.last_start = sm.ws.log_start;
         ss.last_count = sm.ws.log_count;
         ss.seq = sm.ws.seq;
         ss.flushed = flushed;
+    }
+
+    // ---- stage dump: FM (the raw envelope with FM off) of every sample, after the walk and apart from it ----------
+    // From the reset state over [0, N): the host gives a batch with stage arrays one launch over whole streams.
+    if (p.fm_out) {
+        if (lane == 0) {
+            sm.wc.jb.fm_out = p.fm_out + byte0 / SS; // the walk is over: its job can take the dump
+            sm.fm_state = FmState{0, 0, 0};
+        }
+        __syncwarp();
+        for (unsigned long long w0 = 0; w0 < N; w0 += kFmWin)
+            fm_window<SS>(sm.wc.jb, sm, w0, N - w0 < (unsigned long long)kFmWin ? (int)(N - w0) : kFmWin);
     }
 }
 

@@ -38,8 +38,8 @@ def run_gpu(ctx, streams, fmt, rate, freq, fpdm=lib.FPDM_AUTO, block_bytes=0):
     assert lens == padded
     offsets = np.concatenate([[0], np.cumsum(lens)]).astype(np.uint64)
     data = np.concatenate([s.view(np.uint8).ravel() for s in streams]) if streams else np.zeros(0, np.uint8)
-    # Without the stage dump the kernel computes FM on demand (only inside packages, filter state
-    # rebuilt from the previous tile); with it, FM is computed for every tile.  Both must agree.
+    # The walk computes FM on demand either way; a batch with stage arrays adds a pass that makes FM of
+    # every sample after the walk.  Both runs must agree: the stage pass does not disturb the walk.
     ctx.process(data, offsets, fmt, rate, freq, fpdm, block_bytes, want_stages=False)
     ctx.fetch()
     on_demand = [helpers.gpu_stream_results(ctx, i) for i in range(len(streams))]
@@ -48,7 +48,7 @@ def run_gpu(ctx, streams, fmt, rate, freq, fpdm=lib.FPDM_AUTO, block_bytes=0):
     out = []
     for i, s in enumerate(streams):
         r = helpers.gpu_stream_results(ctx, i)
-        d = helpers.compare_results(r, on_demand[i], f"FM on demand vs every tile, stream {i}", stages=False)
+        d = helpers.compare_results(r, on_demand[i], f"without vs with stage arrays, stream {i}", stages=False)
         assert not d, "\n".join(d[:20])
         n = lens[i] // fmt
         r["am"], r["fm"] = ctx.copy_stage(i, n)
@@ -251,8 +251,9 @@ def test_cs8_input_is_cu8_plus_128(ctx, devices):
 
 def test_fm_low_pass_override_and_wrapping_filter(ctx, devices):
     """-Y filter values: a cutoff in Hz, one in us, and a ratio above 0.5 whose feedback coefficient
-    is negative -- the host can then no longer prove the int16 state never wraps, so the kernel
-    variant that is exact by induction alone (up to 31 bracket rounds) runs."""
+    is negative -- the host can then no longer prove the filter monotone, so FM on demand cannot
+    rebuild a window's state by range collapse: the carrier estimate is not deferred, the walk reads
+    FM in order only and makes the windows in between from the last exact state."""
     streams = [synth.ook_stream(41, n_samples=1 << 19, n_bursts=4), synth.ook_stream(42, n_samples=1 << 19, n_bursts=4)]
     try:
         for lp in (25000.0, 12.0, 0.6):

@@ -17,7 +17,7 @@ RATE = 250000
 
 
 def run_skipping(ctx, streams, block_bytes=0, lengths=None):
-    """One batch without stage dumps (the skip is on): per-stream results and the timing counters."""
+    """One cu8 batch without stage arrays: per-stream results and the timing counters."""
     lens = [s.nbytes for s in streams]
     assert all(n % 16 == 0 for n in lens)
     offsets = np.concatenate([[0], np.cumsum(lens)]).astype(np.uint64)
