@@ -124,6 +124,7 @@ typedef struct r433b_timing {
     uint32_t front_repairs;  /* tiles whose start k_detect recomputed (k_front's guess for the tile did not fit) */
     uint32_t idle_skipped;   /* IDLE tiles k_detect ruled out from their summaries without walking them */
     uint32_t idle_rewalks;   /* runs of such tiles walked again because their end state could not be resolved */
+    float grab_ms;           /* k_grab of the last r433b_grab_copy() / r433b_grab_tail() (device time, no copy-out) */
 } r433b_timing;
 
 int r433b_create(int cuda_device, r433b_ctx **out);
@@ -251,6 +252,52 @@ size_t r433b_analysis_text(r433b_ctx const *ctx, r433b_results const *res, uint3
 /* The events of the trial demodulation (compact wire format, see r433b_event_to_bitbuffer). */
 int r433b_analysis_events(r433b_ctx const *ctx, r433b_results const *res, uint32_t package, uint8_t const **events,
         uint32_t *bytes, uint32_t *n_events);
+
+/* ---- signal grabber (`rtl_433 -S all|unknown|known|undecoded`, src/samp_grab.c, src/r_flow.c:345-362) ----------
+   A frame is a run of consecutive block calls of one stream that each return at least one package.  It ends at the
+   first later call that returns none, or at the stream's flush; when the mode selects it, the reference writes the
+   window `samp_grab_write()` cuts out of its ring of everything the run has pushed (R433B_GRAB_RING bytes, never
+   cleared between files).  The run is the used bytes of every stream in batch order, after load-time conversion:
+   cs8 is grabbed as cu8 (+128), cf32 as cs16.  Ring bytes the run never wrote are zero.
+   r433b_grab_plan() emulates the block calls of the fetched batch and lists the files; r433b_grab_copy() gathers
+   their bytes from the batch as it lies on the device (k_grab).  Batch data given with data_on_device must stay
+   valid until the last r433b_grab_copy() of the batch. */
+#define R433B_GRAB_ALL 1       /* grab_mode values of src/rtl_433.c:650-676 */
+#define R433B_GRAB_UNKNOWN 2   /* frames whose packages no decoder decoded (needs a dispatch of every stream) */
+#define R433B_GRAB_KNOWN 3     /* frames with at least one decoded message (idem) */
+#define R433B_GRAB_UNDECODED 4 /* unknown frames pulse_analyzer_check() finds structure in (also needs r433b_analyze) */
+#define R433B_GRAB_RING (12u * 262144u) /* SIGNAL_GRABBER_BUFFER, include/rtl_433.h:22 */
+
+/* What the run pushed before this batch.  NULL prior = the batch starts the run (counter 1, as samp_grab_create()). */
+typedef struct r433b_grab_ring {
+    uint64_t pushed;      /* bytes pushed so far in the run */
+    uint8_t const *tail;  /* host memory: the last min(pushed, R433B_GRAB_RING) of them */
+    uint32_t counter;     /* sg_counter: the next file number to try */
+} r433b_grab_ring;
+
+/* One file samp_grab_write() writes: "g%03u_%gM_%gk.cu8" (or .cs16) with counter, center_frequency / 1e6 and
+   samp_rate / 1e3.  The reference skips names that exist (access()) and counts on: that loop is the caller's, and the
+   counter it ends with is the next batch's prior.counter. */
+typedef struct r433b_grab {
+    uint32_t stream;        /* the stream whose block call ended the frame */
+    uint32_t first_package; /* index into r433b_results.packages of the frame's first package */
+    uint32_t n_packages;    /* packages of the frame */
+    uint32_t grab_len;      /* samples, as printed ("%u samples") */
+    uint32_t bytes;         /* signal_bsize: the file's size */
+    uint32_t counter;       /* prior counter + index of the grab in the batch */
+    int64_t run_end;        /* run byte position at which the window ends (before wrapping in the ring) */
+} r433b_grab;
+
+/* Plan the files of the last fetched batch in `mode` (R433B_GRAB_*).  *grabs points into the context and stays valid
+   until the next plan or batch.  Modes 2-4 need every stream that has packages dispatched (r433b_dispatch*: they
+   record each package's p_events, the run_*_demods() return); mode 4 also needs r433b_analyze(). */
+int r433b_grab_plan(r433b_ctx *ctx, r433b_results const *res, int mode, r433b_grab_ring const *prior,
+        r433b_grab const **grabs, uint32_t *n);
+/* The bytes of grabs [first, first + count) of the last plan back to back into `out` (host, cap bytes). */
+int r433b_grab_copy(r433b_ctx *ctx, r433b_results const *res, uint32_t first, uint32_t count, uint8_t *out, size_t cap);
+/* The next batch's prior: the run's byte count after this batch and its last min(pushed, R433B_GRAB_RING) bytes
+   (`tail` holds R433B_GRAB_RING bytes).  The counter is the caller's (see r433b_grab). */
+int r433b_grab_tail(r433b_ctx *ctx, r433b_results const *res, uint8_t *tail, uint64_t *pushed);
 
 /* ---- pulse-level I/O (SURVEY 8(f4)): packages that never were IQ --------------------------------------
    `rtl_433 -r file.ook` (src/rtl_433.c:1755-1790) and RfRaw test data (-y, src/rtl_433.c:1620-1650) skip the

@@ -8,6 +8,12 @@
 * `python -m rtl_433_b200.captures FILES...` replays capture files through the GPU path and
   prints, per file, the detected packages and the bitbuffer rows every requested device's slicer
   produced, in rtl_433's "{len}hex" notation (what `rtl_433 -R n:vv` logs before decoding).
+* `-S all [--grab-dir DIR]` is the signal grabber (src/samp_grab.c): every frame's IQ is written to
+  `g%03u_%gM_%gk.cu8|.cs16` files as `rtl_433 -S all -r FILES...` writes them.  The grabber's ring runs
+  across the files in processing order, which is group order: the files of each (format, rate,
+  frequency) group in command-line order, groups in the order their first file appears.  That is the
+  command-line order unless groups interleave.  The modes unknown / known / undecoded depend on what the
+  decoders return, so they live behind r433b_dispatch (INTEGRATION.md), not here.
 
 Decoding itself stays with the reference's decoders (INTEGRATION.md); this module stops at the
 bitbuffer like the rest of the package.
@@ -15,6 +21,7 @@ bitbuffer like the rest of the package.
 import argparse
 import os
 import re
+import sys
 
 import numpy as np
 
@@ -208,21 +215,84 @@ def row_code(bb, row):
     return "{%d}%s" % (n, data.hex()[:(n + 3) // 4])
 
 
-def replay(specs, protocols=None, cuda_device=0, max_rows=8, out=print):
-    """Run capture files through the GPU path; report packages and slicer output per file."""
+def grab_name(counter, center_frequency, samp_rate, sample_size):
+    """samp_grab_write()'s file name, src/samp_grab.c:139 (cs8 is grabbed as cu8, cf32 as cs16)."""
+    return "g%03u_%gM_%gk.%s" % (counter, center_frequency / 1e6, samp_rate / 1e3, "cu8" if sample_size == 2 else "cs16")
+
+
+class Grabber:
+    """The run-wide state of `rtl_433 -S`: the ring tail carried from batch to batch, the file counter and the
+    directory the files go to.  Call write() once per batch, in processing order, after ctx.fetch() (and, for the
+    modes that need decoder results, after the dispatch and r433b_analyze)."""
+
+    BLOCK = 128 * 1024
+
+    def __init__(self, directory=".", err=None, page_bytes=256 << 20):
+        self.dir = directory
+        self.err = err if err is not None else sys.stderr
+        self.page = page_bytes
+        self.counter = 1  # samp_grab_create()
+        self.ring = None  # (bytes pushed, tail)
+
+    def write(self, ctx, mode, center_frequency, samp_rate, sample_size):
+        """Write the batch's files; -> their names."""
+        prior = None if self.ring is None else (self.ring[0], self.ring[1], self.counter)
+        plan = ctx.grab_plan(mode, prior)
+        names = []
+        i = 0
+        while i < len(plan):
+            j, total = i, 0
+            while j < len(plan) and (j == i or total + int(plan["bytes"][j]) <= self.page):
+                total += int(plan["bytes"][j])
+                j += 1
+            data = ctx.grab_copy(i, j - i, total)
+            at = 0
+            for g in plan[i:j]:
+                n = int(g["bytes"])
+                names.append(self._file(data[at:at + n], int(g["grab_len"]), center_frequency, samp_rate, sample_size))
+                at += n
+            i = j
+        self.ring = ctx.grab_tail()
+        return names
+
+    def _file(self, data, grab_len, center_frequency, samp_rate, sample_size):
+        wanted = (sample_size * grab_len) & 0xffffffff
+        wanted = (wanted + self.BLOCK - wanted % self.BLOCK) & 0xffffffff
+        if wanted > len(data):
+            self.err.write("Signal bigger than buffer, signal = %u > buffer %u !!\n" % (wanted, len(data)))
+        while True:  # names that exist are skipped, the counter runs on
+            name = grab_name(self.counter, center_frequency, samp_rate, sample_size)
+            self.counter += 1
+            if not os.path.exists(os.path.join(self.dir, name)):
+                break
+        self.err.write("*** Saving signal to file %s (%u samples, %u bytes)\n" % (name, grab_len, len(data)))
+        with open(os.path.join(self.dir, name), "wb") as f:
+            f.write(data.tobytes())
+        return name
+
+
+def replay(specs, protocols=None, cuda_device=0, max_rows=8, out=print, grab_mode=0, grab_dir="."):
+    """Run capture files through the GPU path; report packages and slicer output per file.  grab_mode 1 writes
+    every frame's IQ to grab_dir (`-S all`)."""
     table = lib.default_device_table(include_disabled=True)
     if protocols:
         devs = [d for d in table if d["protocol_num"] in set(protocols)]
     else:
         devs = [d for d in table if d["disabled"] == 0]
+    if grab_mode not in (0, lib.GRAB_ALL):
+        raise ValueError("grab modes unknown / known / undecoded need decoder results: use r433b_grab_plan after r433b_dispatch")
     ctx = lib.Context(cuda_device)
     ctx.set_devices(devs)
+    grabber = Grabber(grab_dir) if grab_mode else None
     summary = []
     try:
         for batch in load_batches(specs):
             ctx.process(batch["data"], batch["offsets"], batch["abi_format"], batch["sample_rate"],
                         batch["center_frequency"], lengths=batch["lengths"])
             res = ctx.fetch()
+            if grabber:
+                ss = {"cu8": 2, "cs8": 2, "cs16": 4, "cf32": 4}[batch["format"]]
+                grabber.write(ctx, grab_mode, batch["center_frequency"], batch["sample_rate"], ss)
             for i, path in enumerate(batch["files"]):
                 pk = res["packages"][res["packages"]["stream"] == i]
                 out(f"{path}: {batch['format']} {batch['sample_rate']} S/s {batch['center_frequency']} Hz, "
@@ -256,8 +326,10 @@ def main(argv=None):
     ap.add_argument("files", nargs="+", help="capture files; rate/frequency/format come from the name as in rtl_433 -r")
     ap.add_argument("-R", dest="protocols", type=int, action="append", help="protocol number(s); default: all enabled")
     ap.add_argument("--device", type=int, default=0)
+    ap.add_argument("-S", dest="grab", choices=["all"], help="signal grabber: write every frame's IQ (rtl_433 -S all)")
+    ap.add_argument("--grab-dir", default=".", help="directory for the grabbed files (default: the current one)")
     a = ap.parse_args(argv)
-    replay(a.files, a.protocols, a.device)
+    replay(a.files, a.protocols, a.device, grab_mode=lib.GRAB_ALL if a.grab else 0, grab_dir=a.grab_dir)
 
 
 if __name__ == "__main__":

@@ -65,6 +65,17 @@ struct HexBuilder {
     }
 };
 
+// pulse_analyzer_check(), src/pulse_analyzer.c:214-276, from the same histograms: 1 when the package has more than
+// one pulse and more than a single pulse width and gap width (the zero-width FSK bin left out), else 0.
+inline int analysis_check(unsigned num_pulses, r433b_analysis const &an)
+{
+    if (num_pulses <= 1) return 0;
+    Histogram pulses = an.hist[0];
+    hist_exchange_sort(pulses, [](HistBin const &a, HistBin const &b) { return a.mean < b.mean; });
+    if (pulses.bins[0].mean == 0) hist_delete(pulses, 0);
+    return pulses.bins_count == 1 && an.hist[1].bins_count == 1 ? 0 : 1;
+}
+
 // What the analyzer concludes for one package.  `pd` must hold the package as the analyzer sees it (levels and
 // estimates filled in); `type` is PULSE_DATA_OOK / _FSK (1 / 2).  Returns the text; fills guess / last_gap.
 inline size_t analysis_finish(struct pulse_data const *pd, int type, r433b_analysis const &an, r433b_guess *guess, char *buf, size_t cap)

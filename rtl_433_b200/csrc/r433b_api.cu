@@ -7,6 +7,7 @@
 #include <cstdlib>
 #include <chrono>
 #include <cstring>
+#include <exception>
 #include <atomic>
 #include <mutex>
 #include <string>
@@ -20,6 +21,7 @@
 #include "r433b_pulses.hpp"
 #include "r433b_analyze.cuh"
 #include "r433b_analyze_host.hpp"
+#include "r433b_grab.cuh"
 
 using namespace r433b;
 
@@ -112,6 +114,19 @@ struct r433b_ctx {
     r433b_batch sub_batch{};
     std::vector<uint64_t> sub_offsets, sub_lengths;
     r433b_results sub_res{};
+    // signal grabber: where the batch's bytes lie on the device, what the dispatch returned per package (sorted
+    // order) and per stream, the last plan and its segments
+    uint8_t const *grab_src = nullptr;
+    unsigned grab_flip = 0;
+    std::vector<uint32_t> p_events;
+    std::vector<uint8_t> dispatched;
+    std::vector<r433b_grab> grabs;
+    std::vector<int64_t> grab_newest; // per grab: bytes the run had pushed when the frame ended
+    bool grab_planned = false;
+    uint64_t grab_pushed = 0;         // run bytes before this batch (prior->pushed)
+    uint64_t grab_prior_bytes = 0;    // of which the device copy of the tail holds the last ones
+    std::vector<uint64_t> grab_cum;   // run offset of stream i within the batch (used bytes), n_streams + 1
+    DevBuf d_grab_prior, d_grab_segs, d_grab_stage;
 };
 
 struct r433b_pulses {
@@ -138,6 +153,9 @@ int fail(r433b_ctx *c, int code, char const *what, cudaError_t e = cudaSuccess)
         cudaError_t e_ = (call);                                   \
         if (e_ != cudaSuccess) return fail(ctx, R433B_ECUDA, #call, e_); \
     } while (0)
+
+// cs8 is read as cu8: the load-time +128 of src/rtl_433.c:1830-1834 is an XOR of every byte's sign bit
+unsigned dp_flip_of(uint32_t sample_format) { return sample_format == R433B_FMT_CS8 ? 0x80808080u : 0u; }
 
 int dev_reserve(r433b_ctx *ctx, DevBuf &b, size_t bytes)
 {
@@ -222,7 +240,8 @@ void r433b_destroy(r433b_ctx *ctx)
     for (DevBuf *b : {&ctx->d_data, &ctx->d_offsets, &ctx->d_train, &ctx->d_pkgs, &ctx->d_ppool, &ctx->d_gpool,
                  &ctx->d_counters, &ctx->d_am, &ctx->d_fm, &ctx->d_devparams, &ctx->d_lists, &ctx->d_pairs,
                  &ctx->d_arena, &ctx->d_cursor, &ctx->d_ranges, &ctx->d_state, &ctx->d_lengths, &ctx->d_stage, &ctx->d_raw, &ctx->d_log, &ctx->d_amoff, &ctx->d_chunks, &ctx->d_tiles,
-                 &ctx->d_order, &ctx->d_an, &ctx->d_an_dev, &ctx->d_an_gap, &ctx->d_an_pairs, &ctx->d_an_arena})
+                 &ctx->d_order, &ctx->d_an, &ctx->d_an_dev, &ctx->d_an_gap, &ctx->d_an_pairs, &ctx->d_an_arena,
+                 &ctx->d_grab_prior, &ctx->d_grab_segs, &ctx->d_grab_stage})
         if (b->p) cudaFree(b->p);
     for (HostBuf *b : {&ctx->h_pkgs, &ctx->h_ppool, &ctx->h_gpool, &ctx->h_pairs, &ctx->h_events, &ctx->h_ranges})
         if (b->p) cudaFreeHost(b->p);
@@ -446,6 +465,9 @@ int r433b_process(r433b_ctx *ctx, r433b_batch const *b)
         if (cf32) ctx->lengths[i] = ctx->lengths[i] / 8 * 4; // whole IQ pairs of floats -> cs16 bytes
     }
     ctx->batch.lengths = ctx->lengths.data();
+    ctx->grabs.clear();
+    ctx->grab_planned = false;
+    ctx->timing.grab_ms = 0;
     uint64_t const total_bytes = b->n_streams ? b->offsets[b->n_streams] / in_div : 0;
     uint64_t used_bytes = 0;
     for (uint64_t v : ctx->lengths) used_bytes += v;
@@ -468,6 +490,8 @@ int r433b_process(r433b_ctx *ctx, r433b_batch const *b)
         if (int r = dev_reserve(ctx, ctx->d_data, total_bytes + 64)) return r;
         d_in = (uint8_t const *)ctx->d_data.p;
     }
+    ctx->grab_src = d_in; // cf32 is grabbed as the cs16 it was converted to
+    ctx->grab_flip = dp_flip_of(b->sample_format);
     if (cf32 && !b->data_on_device)
         if (int r = dev_reserve(ctx, ctx->d_raw, 2 * total_bytes + 64)) return r;
     if (int r = dev_reserve(ctx, ctx->d_offsets, (b->n_streams + 1) * sizeof(uint64_t))) return r;
@@ -504,7 +528,7 @@ int r433b_process(r433b_ctx *ctx, r433b_batch const *b)
     dp.first_chunk = 1;
     dp.state = nullptr;
     dp.use_mag = ctx->use_mag;
-    dp.flip = b->sample_format == R433B_FMT_CS8 ? 0x80808080u : 0u;
+    dp.flip = dp_flip_of(b->sample_format);
     dp.enable_fm = ctx->enable_fm;
     dp.fpdm = (int)ctx->fpdm;
     dp.rate = b->samp_rate;
@@ -871,6 +895,8 @@ int r433b_fetch(r433b_ctx *ctx, r433b_results *out)
         for (uint32_t i = 0; i < ctx->n_pkgs; ++i) sorted[i] = pk[ix[i]];
         if (ctx->n_pkgs) memcpy(pk, sorted.data(), (size_t)ctx->n_pkgs * sizeof(r433b_package));
         ctx->analyzed = false;
+        ctx->p_events.assign(ctx->n_pkgs, 0);
+        ctx->dispatched.assign(ctx->batch.n_streams, 0);
     }
     ctx->fetched = true;
     out->n_packages = ctx->n_pkgs;
@@ -1029,7 +1055,9 @@ int replay_stream(r433b_ctx *ctx, r433b_results const *res, uint32_t stream, Per
                 }
             }
         }
+        if (pi < ctx->p_events.size()) ctx->p_events[pi] = (uint32_t)p_events;
     }
+    if (stream < ctx->dispatched.size()) ctx->dispatched[stream] = 1;
     return R433B_OK;
 }
 
@@ -1235,6 +1263,7 @@ int r433b_process_pulses(r433b_ctx *ctx, r433b_pulses const *ps)
     ctx->processed = ctx->fetched = false;
     ctx->d2h_done = false;
     ctx->pulse_mode = true;
+    ctx->grab_planned = false;
     ctx->pulse_meta = set.pk;
     ctx->batch = r433b_batch{};
     ctx->batch.sample_format = 2;
@@ -1493,6 +1522,233 @@ int r433b_wait(r433b_ctx *ctx, r433b_results *out)
     ctx->in_flight = false;
     if (!ctx->worker_rc && out) *out = ctx->sub_res;
     return ctx->worker_rc;
+}
+
+} // extern "C"
+
+
+// ------------------------------------------------ signal grabber (src/samp_grab.c, src/r_flow.c:345-362) ------
+
+namespace {
+
+// The run byte range [a, b) as segments of the staging buffer from `dst` on: negative positions were never written
+// (zero), positions before the batch come from the device copy of the prior tail, the rest from the streams' used
+// bytes as they lie on the device.
+void grab_segments(r433b_ctx const *ctx, int64_t a, int64_t b, uint64_t &dst, std::vector<GrabSeg> &segs)
+{
+    int64_t const pushed = (int64_t)ctx->grab_pushed;
+    while (a < b) {
+        GrabSeg g{};
+        g.dst = dst;
+        int64_t e;
+        if (a < 0) {
+            e = std::min<int64_t>(b, 0);
+            g.kind = kGrabZero;
+        } else if (a < pushed) {
+            e = std::min<int64_t>(b, pushed);
+            g.kind = kGrabPrior;
+            g.src = (uint64_t)(a - (pushed - (int64_t)ctx->grab_prior_bytes));
+        } else {
+            uint64_t const u = (uint64_t)(a - pushed);
+            std::vector<uint64_t> const &cum = ctx->grab_cum;
+            size_t const s = (size_t)(std::upper_bound(cum.begin(), cum.end(), u) - cum.begin()) - 1;
+            e = std::min<int64_t>(b, pushed + (int64_t)cum[s + 1]);
+            g.kind = kGrabBatch;
+            g.src = ctx->offsets[s] + (u - cum[s]);
+        }
+        g.len = (uint64_t)(e - a);
+        segs.push_back(g);
+        dst += g.len;
+        a = e;
+    }
+}
+
+// k_grab over `segs` (covering [0, total)) into the staging buffer, then one copy to `out`
+int grab_gather(r433b_ctx *ctx, std::vector<GrabSeg> const &segs, uint64_t total, uint8_t *out)
+{
+    if (!total) return R433B_OK;
+    cudaStream_t const st = 0;
+    uint64_t const staged = (total + kGrabSpan - 1) / kGrabSpan * kGrabSpan;
+    if (int r = dev_reserve(ctx, ctx->d_grab_segs, segs.size() * sizeof(GrabSeg))) return r;
+    if (int r = dev_reserve(ctx, ctx->d_grab_stage, staged)) return r;
+    CU(cudaMemcpyAsync(ctx->d_grab_segs.p, segs.data(), segs.size() * sizeof(GrabSeg), cudaMemcpyHostToDevice, st));
+    GrabParams gp{};
+    gp.batch = ctx->grab_src;
+    gp.prior = (uint8_t const *)ctx->d_grab_prior.p;
+    gp.segs = (GrabSeg const *)ctx->d_grab_segs.p;
+    gp.n_segs = (unsigned)segs.size();
+    gp.flip = ctx->grab_flip;
+    gp.total = total;
+    gp.out = (uint4 *)ctx->d_grab_stage.p;
+    uint64_t const warps = staged / kGrabSpan;
+    unsigned const grid = (unsigned)((warps * 32 + kGrabThreads - 1) / kGrabThreads);
+    CU(cudaEventRecord(ctx->ev[0], st));
+    R4_LAUNCH(k_grab, grid, kGrabThreads, 0, st, gp);
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(ctx->ev[1], st));
+    CU(cudaMemcpy(out, ctx->d_grab_stage.p, total, cudaMemcpyDeviceToHost));
+    cudaEventElapsedTime(&ctx->timing.grab_ms, ctx->ev[0], ctx->ev[1]);
+    return R433B_OK;
+}
+
+} // namespace
+
+extern "C" {
+
+int r433b_grab_plan(r433b_ctx *ctx, r433b_results const *res, int mode, r433b_grab_ring const *prior,
+        r433b_grab const **grabs, uint32_t *n)
+{
+    try {
+        if (!ctx || !res || !grabs || !n) return fail(ctx, R433B_EINVAL, "null argument");
+        if (mode < R433B_GRAB_ALL || mode > R433B_GRAB_UNDECODED) return fail(ctx, R433B_EINVAL, "grab mode must be 1 .. 4");
+        if (prior && prior->pushed && !prior->tail) return fail(ctx, R433B_EINVAL, "prior ring without its tail");
+        if (!ctx->fetched) return fail(ctx, R433B_ESTATE, "r433b_grab_plan before r433b_fetch");
+        if (ctx->pulse_mode) return fail(ctx, R433B_ESTATE, "a batch of loaded pulse data has no IQ to grab");
+        if (res->packages != (r433b_package const *)ctx->h_pkgs.p || res->n_packages != ctx->n_pkgs)
+            return fail(ctx, R433B_EINVAL, "results are not the context's last fetched batch");
+        if (mode != R433B_GRAB_ALL)
+            for (uint32_t i = 0; i < res->n_packages; ++i)
+                if (!ctx->dispatched[res->packages[i].stream])
+                    return fail(ctx, R433B_ESTATE, "grab modes 2-4 need every stream with packages dispatched first");
+        if (mode == R433B_GRAB_UNDECODED && !ctx->analyzed)
+            return fail(ctx, R433B_ESTATE, "grab mode 4 (undecoded) needs r433b_analyze() first");
+        CU(cudaSetDevice(ctx->device));
+        uint32_t const S = R433B_GRAB_RING;
+        uint64_t const pushed = prior ? prior->pushed : 0;
+        uint64_t const tail = std::min<uint64_t>(pushed, S);
+        if (int r = dev_reserve(ctx, ctx->d_grab_prior, tail + 16)) return r;
+        if (tail) CU(cudaMemcpy(ctx->d_grab_prior.p, prior->tail, tail, cudaMemcpyHostToDevice));
+        ctx->grab_pushed = pushed;
+        ctx->grab_prior_bytes = tail;
+        uint32_t const n_streams = ctx->batch.n_streams;
+        ctx->grab_cum.assign(n_streams + 1, 0);
+        for (uint32_t i = 0; i < n_streams; ++i) ctx->grab_cum[i + 1] = ctx->grab_cum[i] + ctx->lengths[i];
+        ctx->grabs.clear();
+        ctx->grab_newest.clear();
+
+        // the block calls of push_sdr_flow(), stream by stream (src/rtl_433.c:1797-1854, src/r_flow.c:137-147, :245-362);
+        // the frame state is per file (reset_sdr_flow(), src/r_flow.c:79-97), the ring and the counter are per run
+        uint32_t const SS = ctx->batch.sample_format, B = ctx->batch.block_bytes;
+        uint32_t counter = prior ? prior->counter : 1; // samp_grab_create() starts at 1
+        r433b_package const *pk = res->packages;
+        uint32_t k = 0;
+        for (uint32_t s = 0; s < n_streams; ++s) {
+            uint64_t const L = ctx->lengths[s], base = pushed + ctx->grab_cum[s];
+            uint64_t const n_blocks = (L + B - 1) / B; // block n_blocks is the flush
+            uint32_t start_ago = 0, end_ago = 0, quality = 0, first = 0;
+            uint64_t events = 0;
+            while (k < res->n_packages && pk[k].stream < s) ++k;
+            for (uint64_t blk = 0; blk <= n_blocks; ++blk) {
+                bool const here = k < res->n_packages && pk[k].stream == s && (uint64_t)pk[k].block == blk;
+                if (!start_ago && !here) { // no frame and no package: nothing but ageing until the next package
+                    if (k < res->n_packages && pk[k].stream == s && (uint64_t)pk[k].block > blk) blk = (uint64_t)pk[k].block - 1;
+                    else break;
+                    continue;
+                }
+                uint64_t const len = blk < n_blocks ? std::min<uint64_t>(B, L - blk * B) : 0;
+                uint32_t const n_samples = (uint32_t)(len / SS);
+                uint64_t const P = base + std::min<uint64_t>(L, blk * B + len); // pushed after this call's push
+                if (start_ago) start_ago += n_samples;
+                if (end_ago) end_ago += n_samples;
+                uint64_t d_events = 0;
+                for (; k < res->n_packages && pk[k].stream == s && (uint64_t)pk[k].block == blk; ++k) {
+                    if (!start_ago) {
+                        start_ago = pk[k].start_ago;
+                        first = k;
+                    }
+                    end_ago = pk[k].end_ago;
+                    uint32_t const pe = ctx->p_events[k];
+                    d_events += pe;
+                    if (mode == R433B_GRAB_UNDECODED && pe == 0) {
+                        uint32_t const q = (uint32_t)analysis_check(pk[k].num_pulses, ctx->an[ctx->dev_index[k]]);
+                        if (q > quality) quality = q;
+                    }
+                }
+                events += d_events;
+                if (!(start_ago && end_ago > n_samples)) continue;
+                bool const take = mode == R433B_GRAB_ALL || (mode == R433B_GRAB_UNKNOWN && events == 0)
+                        || (mode == R433B_GRAB_KNOWN && events > 0) || (mode == R433B_GRAB_UNDECODED && events == 0 && quality > 0);
+                if (take) {
+                    // unsigned arithmetic of src/r_flow.c:352-356 and samp_grab_write(), src/samp_grab.c:98-134
+                    uint32_t const pad = n_samples / 8;
+                    uint32_t const start_padded = start_ago + pad, end_padded = end_ago - pad;
+                    uint32_t const grab_len = start_padded - end_padded;
+                    uint32_t bsize = SS * grab_len;
+                    bsize += 131072u - bsize % 131072u;
+                    uint32_t const sg_len = (uint32_t)std::min<uint64_t>(P, S);
+                    if (bsize > sg_len) bsize = sg_len;
+                    uint32_t const sg_index = (uint32_t)(P % S);
+                    uint32_t end_pos = SS * end_padded;
+                    end_pos = sg_index >= end_pos ? sg_index - end_pos : S - end_pos + sg_index;
+                    uint64_t const back = ((uint64_t)sg_index + S - end_pos % S) % S; // bytes between window end and newest
+                    r433b_grab g{};
+                    g.stream = s;
+                    g.first_package = first;
+                    g.n_packages = k - first;
+                    g.grab_len = grab_len;
+                    g.bytes = bsize;
+                    g.counter = counter++;
+                    g.run_end = (int64_t)P - (int64_t)back;
+                    ctx->grabs.push_back(g);
+                    ctx->grab_newest.push_back((int64_t)P);
+                }
+                start_ago = 0;
+                events = 0;
+                quality = 0;
+            }
+        }
+        ctx->grab_planned = true;
+        *grabs = ctx->grabs.data();
+        *n = (uint32_t)ctx->grabs.size();
+        return R433B_OK;
+    } catch (std::exception const &) { // allocation failures of the host vectors
+        return fail(ctx, R433B_ENOMEM, "r433b_grab_plan: out of host memory");
+    }
+}
+
+int r433b_grab_copy(r433b_ctx *ctx, r433b_results const *res, uint32_t first, uint32_t count, uint8_t *out, size_t cap)
+{
+    try {
+        if (!ctx || !res) return fail(ctx, R433B_EINVAL, "null argument");
+        if (!ctx->grab_planned) return fail(ctx, R433B_ESTATE, "r433b_grab_copy before r433b_grab_plan");
+        if ((uint64_t)first + count > ctx->grabs.size()) return fail(ctx, R433B_EINVAL, "grab index out of range");
+        CU(cudaSetDevice(ctx->device));
+        uint64_t dst = 0;
+        std::vector<GrabSeg> segs;
+        for (uint32_t i = first; i < first + count; ++i) {
+            r433b_grab const &g = ctx->grabs[i];
+            int64_t const lo = g.run_end - (int64_t)g.bytes, hi = g.run_end;
+            // positions older than the ring holds read its newest bytes at the same slots (one wrap at most: bytes <= ring)
+            int64_t const oldest = ctx->grab_newest[i] - (int64_t)R433B_GRAB_RING;
+            if (lo < oldest) {
+                grab_segments(ctx, lo + (int64_t)R433B_GRAB_RING, std::min<int64_t>(hi, oldest) + (int64_t)R433B_GRAB_RING, dst, segs);
+                grab_segments(ctx, oldest, hi, dst, segs);
+            } else
+                grab_segments(ctx, lo, hi, dst, segs);
+        }
+        if (dst > cap || (dst && !out)) return fail(ctx, R433B_EINVAL, "output buffer smaller than the grabs' bytes");
+        return grab_gather(ctx, segs, dst, out);
+    } catch (std::exception const &) { // allocation failures of the host vectors
+        return fail(ctx, R433B_ENOMEM, "r433b_grab_copy: out of host memory");
+    }
+}
+
+int r433b_grab_tail(r433b_ctx *ctx, r433b_results const *res, uint8_t *tail, uint64_t *pushed)
+{
+    try {
+        if (!ctx || !res || !tail || !pushed) return fail(ctx, R433B_EINVAL, "null argument");
+        if (!ctx->grab_planned) return fail(ctx, R433B_ESTATE, "r433b_grab_tail before r433b_grab_plan");
+        CU(cudaSetDevice(ctx->device));
+        int64_t const end = (int64_t)(ctx->grab_pushed + ctx->grab_cum.back());
+        int64_t const begin = std::max<int64_t>(0, end - (int64_t)R433B_GRAB_RING);
+        uint64_t dst = 0;
+        std::vector<GrabSeg> segs;
+        grab_segments(ctx, begin, end, dst, segs);
+        *pushed = (uint64_t)end;
+        return grab_gather(ctx, segs, dst, tail);
+    } catch (std::exception const &) { // allocation failures of the host vectors
+        return fail(ctx, R433B_ENOMEM, "r433b_grab_tail: out of host memory");
+    }
 }
 
 } // extern "C"

@@ -31,7 +31,7 @@ EXPORTS = ["r433b_create", "r433b_destroy", "r433b_last_error", "r433b_set_level
            "r433b_format_ook", "r433b_format_ook_header", "r433b_format_vcd", "r433b_format_vcd_header",
            "r433b_dump_logic_u8", "r433b_set_gates", "r433b_get_gated",
            "r433b_dispatch_r_devices_parallel", "r433b_analyze", "r433b_analysis_get", "r433b_analysis_text",
-           "r433b_analysis_events", "r433b_submit", "r433b_wait"]
+           "r433b_analysis_events", "r433b_submit", "r433b_wait", "r433b_grab_plan", "r433b_grab_copy", "r433b_grab_tail"]
 
 
 def build(force=False, verbose=False):
@@ -110,7 +110,21 @@ class Timing(C.Structure):
     _fields_ = [("h2d_ms", C.c_float), ("detect_ms", C.c_float), ("slice_ms", C.c_float), ("d2h_ms", C.c_float),
                 ("total_ms", C.c_float), ("detect_launches", C.c_uint32), ("slice_launches", C.c_uint32),
                 ("front_ms", C.c_float), ("front_launches", C.c_uint32), ("front_redone", C.c_uint32),
-                ("front_repairs", C.c_uint32), ("idle_skipped", C.c_uint32), ("idle_rewalks", C.c_uint32)]
+                ("front_repairs", C.c_uint32), ("idle_skipped", C.c_uint32), ("idle_rewalks", C.c_uint32),
+                ("grab_ms", C.c_float)]
+
+
+GRAB_ALL, GRAB_UNKNOWN, GRAB_KNOWN, GRAB_UNDECODED = 1, 2, 3, 4
+GRAB_RING = 12 * 262144  # SIGNAL_GRABBER_BUFFER
+
+
+class GrabRing(C.Structure):
+    _fields_ = [("pushed", C.c_uint64), ("tail", C.c_void_p), ("counter", C.c_uint32)]
+
+
+GRAB_DTYPE = np.dtype([("stream", "<u4"), ("first_package", "<u4"), ("n_packages", "<u4"), ("grab_len", "<u4"),
+                       ("bytes", "<u4"), ("counter", "<u4"), ("run_end", "<i8")])
+assert GRAB_DTYPE.itemsize == 32
 
 
 class PulseData(C.Structure):
@@ -172,6 +186,10 @@ def load():
     L.r433b_analysis_events.argtypes = [C.c_void_p, C.POINTER(Results), C.c_uint32, C.POINTER(C.c_void_p), C.POINTER(C.c_uint32),
                                         C.POINTER(C.c_uint32)]
     L.r433b_set_gates.argtypes = [C.c_void_p, C.POINTER(Gate), C.c_uint32]
+    L.r433b_grab_plan.argtypes = [C.c_void_p, C.POINTER(Results), C.c_int, C.POINTER(GrabRing), C.POINTER(C.c_void_p),
+                                  C.POINTER(C.c_uint32)]
+    L.r433b_grab_copy.argtypes = [C.c_void_p, C.POINTER(Results), C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t]
+    L.r433b_grab_tail.argtypes = [C.c_void_p, C.POINTER(Results), C.c_void_p, C.POINTER(C.c_uint64)]
     L.r433b_get_gated.restype = C.c_uint64
     L.r433b_get_gated.argtypes = [C.c_void_p]
     L.r433b_pulses_create.restype = C.c_void_p
@@ -473,6 +491,35 @@ class Context:
         fm = np.zeros(n, np.int16)
         got = self._check(self.L.r433b_copy_stage(self.h, stream, am.ctypes.data, fm.ctypes.data, n))
         return am[:got], fm[:got]
+
+    def grab_plan(self, mode, prior=None):
+        """The signal grabber's files for the fetched batch (include/r433b.h: r433b_grab_plan) -> GRAB_DTYPE array.
+        `prior` = (pushed, tail bytes, counter) of the run before this batch, or None when the batch starts it."""
+        ring = None
+        if prior is not None:
+            pushed, tail, counter = prior
+            tail = np.ascontiguousarray(tail, dtype=np.uint8)
+            ring = GrabRing(pushed, tail.ctypes.data if tail.size else None, counter)
+            self._grab_keep = tail
+        ptr, n = C.c_void_p(), C.c_uint32()
+        self._check(self.L.r433b_grab_plan(self.h, C.byref(self._res), mode, C.byref(ring) if ring is not None else None,
+                                           C.byref(ptr), C.byref(n)))
+        if not n.value:
+            return np.zeros(0, GRAB_DTYPE)
+        return np.frombuffer((C.c_uint8 * (n.value * GRAB_DTYPE.itemsize)).from_address(ptr.value), dtype=GRAB_DTYPE).copy()
+
+    def grab_copy(self, first, count, nbytes):
+        """The bytes of grabs [first, first + count) of the last plan, back to back (nbytes = their sum)."""
+        out = np.zeros(max(int(nbytes), 1), np.uint8)
+        self._check(self.L.r433b_grab_copy(self.h, C.byref(self._res), first, count, out.ctypes.data, int(nbytes)))
+        return out[:int(nbytes)]
+
+    def grab_tail(self):
+        """-> (bytes pushed by the run after this batch, its last min(pushed, GRAB_RING) bytes): the next prior."""
+        out = np.zeros(GRAB_RING, np.uint8)
+        pushed = C.c_uint64()
+        self._check(self.L.r433b_grab_tail(self.h, C.byref(self._res), out.ctypes.data, C.byref(pushed)))
+        return pushed.value, out[:min(pushed.value, GRAB_RING)]
 
     def pulse_data(self, package_index):
         pd = PulseData()
