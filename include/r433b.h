@@ -125,6 +125,8 @@ typedef struct r433b_timing {
     uint32_t idle_skipped;   /* IDLE tiles k_detect ruled out from their summaries without walking them */
     uint32_t idle_rewalks;   /* runs of such tiles walked again because their end state could not be resolved */
     float grab_ms;           /* k_grab of the last r433b_grab_copy() / r433b_grab_tail() (device time, no copy-out) */
+    uint32_t chain_folds;       /* chained batches: chunk ends that folded a deferred carrier-estimate log ... */
+    uint32_t chain_fm_rebuilds; /* ... and that made the FM filter state exact at the chunk end */
 } r433b_timing;
 
 int r433b_create(int cuda_device, r433b_ctx **out);
@@ -166,6 +168,38 @@ int r433b_set_gates(r433b_ctx *ctx, r433b_gate const *gates, uint32_t n);
 /* rtl_433 -r on every stream of the batch: block loop, flush, reset (src/rtl_433.c:1797-1854),
    then all slicers on every package.  Synchronous; results stay on the device until fetched. */
 int r433b_process(r433b_ctx *ctx, r433b_batch const *batch);
+/* ---- chained batches: files longer than one batch, corpora larger than memory, buffers as they arrive ----------
+   The reference pushes a file through push_sdr_flow() one block at a time and carries O(1) state between the calls
+   (src/rtl_433.c:1827).  A chain does the same for the streams of consecutive batches: slot i of the chain carries the
+   demodulator state of one file from one r433b_process_chained() call to the next.
+
+   The rule: cut a file into chunks at whole-block boundaries and pass them, in order, as stream i of consecutive
+   chained batches.  The results equal those of the uncut file: every r433b_package field, the pulse and gap widths,
+   every pair and event byte, the stage arrays (each chunk's part), the analyzer text, and the decoders' output and
+   statistics.
+   - Every chunk but a file's last holds a whole number of blocks: a multiple of block_bytes input bytes (2 x
+     block_bytes for cf32).  Other lengths return R433B_EINVAL.
+   - last[i] != 0: the file ends with this chunk (the flush runs); the slot then starts a new file, as `rtl_433 -r a
+     -r b` does: its next chunk starts from the reset state with seq 0.  An empty chunk that is not the last changes
+     nothing; an empty last chunk only flushes.
+   - Packages report absolute offset, end_pos and block; seq continues across chunks; r433b_package_file_pos() gives
+     the uncut file's sample_file_pos.  fetch, dispatch*, analyze, digests and gates work on a chained batch unchanged.
+   - While any slot is inside a file, the sample format, rate, centre frequency (and so FPDM), block size, levels,
+     FM low-pass and whether FM is on (which follows from the devices) must not change: R433B_ESTATE.  A batch whose
+     n_streams differs from the chain's returns R433B_EINVAL.  r433b_grab_plan() on a chained batch returns R433B_ESTATE.
+   - A chain belongs to the context that created it and owns its device memory: per slot the carried state, the
+     pulse-train scratch (19.2 KB) and a copy of both (a batch whose result arenas overflow runs again from it), about
+     40 KB per slot.  r433b_destroy() frees the device memory of the context's chains; such a chain only accepts
+     r433b_chain_destroy().  After a failed r433b_process_chained() the chain is undefined. */
+typedef struct r433b_chain r433b_chain;
+/* every slot at a file start */
+int r433b_chain_create(r433b_ctx *ctx, uint32_t n_streams, r433b_chain **out);
+void r433b_chain_destroy(r433b_chain *chain);
+/* batch stream i is the next chunk of slot i; last[i] != 0: the file ends with it (flush, then a new file) */
+int r433b_process_chained(r433b_ctx *ctx, r433b_batch const *batch, r433b_chain *chain, uint8_t const *last);
+/* absolute sample index of the first sample of slot i's chunk in the last chained batch */
+int r433b_chain_base(r433b_chain const *chain, uint32_t stream, uint64_t *first_sample);
+
 /* Copy the compact results to host memory owned by the context. */
 int r433b_fetch(r433b_ctx *ctx, r433b_results *out);
 int r433b_get_timing(r433b_ctx const *ctx, r433b_timing *out);

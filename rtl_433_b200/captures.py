@@ -8,6 +8,9 @@
 * `python -m rtl_433_b200.captures FILES...` replays capture files through the GPU path and
   prints, per file, the detected packages and the bitbuffer rows every requested device's slicer
   produced, in rtl_433's "{len}hex" notation (what `rtl_433 -R n:vv` logs before decoding).
+* `--chunk-mb N` streams every group through a chain (r433b_process_chained): each call reads the next N MiB of
+  whole blocks of every file at an offset, so host memory is about (files in the group) x N MiB; the printed
+  output is that of the plain run.  It does not combine with `-S`.
 * `-S all [--grab-dir DIR]` is the signal grabber (src/samp_grab.c): every frame's IQ is written to
   `g%03u_%gM_%gk.cu8|.cs16` files as `rtl_433 -S all -r FILES...` writes them.  The grabber's ring runs
   across the files in processing order, which is group order: the files of each (format, rate,
@@ -271,9 +274,106 @@ class Grabber:
         return name
 
 
-def replay(specs, protocols=None, cuda_device=0, max_rows=8, out=print, grab_mode=0, grab_dir="."):
+def _file_rows(ctx, res, i, devs, protocols, max_rows):
+    """What one stream of a fetched batch adds to its file's report: package lines, every event's row text (None when
+    the event is not shown) in dispatch order."""
+    pk = res["packages"][res["packages"]["stream"] == i]
+    events = []
+
+    def on_event(pkg, dev, pd, bb, events=events):
+        events.append((pkg, dev, bb.copy()))
+        return 0
+
+    ctx.dispatch(i, on_event)
+    lines = []
+    for k in pk:
+        kind = "OOK" if k["type"] == lib.PACKAGE_OOK else "FSK"
+        lines.append(f"  {kind} package @{int(k['offset'])}: {int(k['num_pulses'])} pulses, "
+                     f"levels low {int(k['ook_low_estimate'])} high {int(k['ook_high_estimate'])}")
+    rows = []
+    for pkg, dev, bb in events:
+        shown = protocols or any(int(b) > 16 for b in bb["bits_per_row"][:int(bb["num_rows"])])
+        rows.append(f"    [{devs[dev]['protocol_num']}] {devs[dev]['name']}: "
+                    + " ".join(row_code(bb, r) for r in range(min(int(bb["num_rows"]), max_rows))) if shown else None)
+    return len(pk), lines, rows
+
+
+def _print_file(out, path, batch, n_samples, rep):
+    n_pk, lines, rows = rep
+    out(f"{path}: {batch['format']} {batch['sample_rate']} S/s {batch['center_frequency']} Hz, "
+        f"{n_samples} samples, {n_pk} package(s)")
+    for line in lines:
+        out(line)
+    for line in [r for r in rows if r is not None][:40]:
+        out(line)
+    return {"file": path, "packages": n_pk, "events": len(rows)}
+
+
+_IN_BYTES = {lib.FMT_CU8: 2, lib.FMT_CS8: 2, lib.FMT_CS16: 4, lib.FMT_CF32: 8}
+
+
+def _chunked_groups(specs, default_rate=DEFAULT_RATE, default_freq=DEFAULT_FREQ):
+    """The groups of load_batches() without their data: per file a reader of (offset, count) bytes and its length."""
+    groups = {}
+    for spec in specs:
+        info = parse_capture_name(spec)
+        if info["content"] == "sigmf":
+            sm = read_sigmf(info["path"])
+            key, src = ("cu8", sm["sample_rate"], sm["center_frequency"]), sm["data"]
+        else:
+            if info["format"] not in _ABI_FORMAT:
+                raise ValueError(f"{spec}: format {info['format']!r} is not on the GPU path (cu8, cs8, cs16, cf32 are)")
+            key, src = (info["format"], info["sample_rate"] or default_rate, info["center_frequency"] or default_freq), None
+        groups.setdefault(key, []).append((info["path"], src))
+    out = []
+    for (fmt, rate, freq), files in groups.items():
+        ss = _IN_BYTES[_ABI_FORMAT[fmt]]
+        sizes = [len(src) if src is not None else os.path.getsize(p) for p, src in files]
+        out.append({"format": fmt, "abi_format": _ABI_FORMAT[fmt], "sample_rate": rate, "center_frequency": freq,
+                    "files": [p for p, _ in files], "sources": [src for _, src in files],
+                    "lengths": np.array([n // ss * ss for n in sizes], np.uint64)})
+    return out
+
+
+def _replay_chunked(ctx, batch, chunk_mb, report):
+    """One group through a chain: every round reads the next `chunk_mb` MiB of whole blocks of every file at an
+    offset, so host memory is about (files in the group) x chunk_mb MiB.  -> per file the merged report."""
+    block = 262144 * (2 if batch["abi_format"] == lib.FMT_CF32 else 1)  # DEFAULT_BUF_LENGTH, of cs16 for cf32
+    step = max(1, (chunk_mb << 20) // block) * block
+    n = len(batch["files"])
+    lengths = [int(v) for v in batch["lengths"]]
+    reps = [(0, [], []) for _ in range(n)]
+    chain = lib.Chain(ctx, n)
+    try:
+        for r in range((max(lengths) + step - 1) // step if max(lengths) else 1):
+            at = r * step
+            data = np.zeros(n * step, np.uint8)
+            lens, last, live = [], [], []
+            for i, (path, src) in enumerate(zip(batch["files"], batch["sources"])):
+                take = max(0, min(step, lengths[i] - at))
+                if take:
+                    data[i * step:i * step + take] = (src[at:at + take] if src is not None
+                                                       else np.fromfile(path, dtype=np.uint8, count=take, offset=at))
+                live.append(at < lengths[i] or (at == 0 and lengths[i] == 0))
+                lens.append(take)
+                last.append(1 if at + take >= lengths[i] else 0)
+            offsets = np.arange(n + 1, dtype=np.uint64) * np.uint64(step)
+            ctx.process(data, offsets, batch["abi_format"], batch["sample_rate"], batch["center_frequency"],
+                        lengths=lens, chain=chain, last=last)
+            res = ctx.fetch()
+            for i in range(n):
+                if live[i]:
+                    k, lines, rows = report(res, i)
+                    reps[i] = (reps[i][0] + k, reps[i][1] + lines, reps[i][2] + rows)
+    finally:
+        chain.close()
+    return reps
+
+
+def replay(specs, protocols=None, cuda_device=0, max_rows=8, out=print, grab_mode=0, grab_dir=".", chunk_mb=0):
     """Run capture files through the GPU path; report packages and slicer output per file.  grab_mode 1 writes
-    every frame's IQ to grab_dir (`-S all`)."""
+    every frame's IQ to grab_dir (`-S all`).  chunk_mb > 0 streams every group through a chain, chunk_mb MiB of every
+    file per call: the report is the same, host memory stays bounded."""
     table = lib.default_device_table(include_disabled=True)
     if protocols:
         devs = [d for d in table if d["protocol_num"] in set(protocols)]
@@ -281,41 +381,29 @@ def replay(specs, protocols=None, cuda_device=0, max_rows=8, out=print, grab_mod
         devs = [d for d in table if d["disabled"] == 0]
     if grab_mode not in (0, lib.GRAB_ALL):
         raise ValueError("grab modes unknown / known / undecoded need decoder results: use r433b_grab_plan after r433b_dispatch")
+    if grab_mode and chunk_mb:
+        raise ValueError("the signal grabber does not run on chained batches (-S with --chunk-mb)")
     ctx = lib.Context(cuda_device)
     ctx.set_devices(devs)
     grabber = Grabber(grab_dir) if grab_mode else None
     summary = []
     try:
-        for batch in load_batches(specs):
-            ctx.process(batch["data"], batch["offsets"], batch["abi_format"], batch["sample_rate"],
-                        batch["center_frequency"], lengths=batch["lengths"])
-            res = ctx.fetch()
-            if grabber:
-                ss = {"cu8": 2, "cs8": 2, "cs16": 4, "cf32": 4}[batch["format"]]
-                grabber.write(ctx, grab_mode, batch["center_frequency"], batch["sample_rate"], ss)
+        groups = _chunked_groups(specs) if chunk_mb else load_batches(specs)
+        for batch in groups:
+            if chunk_mb:
+                reps = _replay_chunked(ctx, batch, chunk_mb,
+                                       lambda res, i: _file_rows(ctx, res, i, devs, protocols, max_rows))
+            else:
+                ctx.process(batch["data"], batch["offsets"], batch["abi_format"], batch["sample_rate"],
+                            batch["center_frequency"], lengths=batch["lengths"])
+                res = ctx.fetch()
+                if grabber:
+                    ss = {"cu8": 2, "cs8": 2, "cs16": 4, "cf32": 4}[batch["format"]]
+                    grabber.write(ctx, grab_mode, batch["center_frequency"], batch["sample_rate"], ss)
+                reps = [_file_rows(ctx, res, i, devs, protocols, max_rows) for i in range(len(batch["files"]))]
             for i, path in enumerate(batch["files"]):
-                pk = res["packages"][res["packages"]["stream"] == i]
-                out(f"{path}: {batch['format']} {batch['sample_rate']} S/s {batch['center_frequency']} Hz, "
-                    f"{int(batch['lengths'][i]) // {lib.FMT_CU8: 2, lib.FMT_CS8: 2, lib.FMT_CS16: 4, lib.FMT_CF32: 8}[batch['abi_format']]} samples, {len(pk)} package(s)")
-                events = []
-
-                def on_event(pkg, dev, pd, bb, events=events):
-                    events.append((pkg, dev, bb.copy()))
-                    return 0
-
-                ctx.dispatch(i, on_event)
-                for k in pk:
-                    kind = "OOK" if k["type"] == lib.PACKAGE_OOK else "FSK"
-                    out(f"  {kind} package @{int(k['offset'])}: {int(k['num_pulses'])} pulses, "
-                        f"levels low {int(k['ook_low_estimate'])} high {int(k['ook_high_estimate'])}")
-                shown = 0
-                for pkg, dev, bb in events:
-                    rows = [row_code(bb, r) for r in range(min(int(bb["num_rows"]), max_rows))]
-                    if protocols or any(int(b) > 16 for b in bb["bits_per_row"][:int(bb["num_rows"])]):
-                        if shown < 40:
-                            out(f"    [{devs[dev]['protocol_num']}] {devs[dev]['name']}: " + " ".join(rows))
-                        shown += 1
-                summary.append({"file": path, "packages": len(pk), "events": len(events)})
+                n_samples = int(batch["lengths"][i]) // _IN_BYTES[batch["abi_format"]]
+                summary.append(_print_file(out, path, batch, n_samples, reps[i]))
     finally:
         ctx.close()
     return summary
@@ -328,8 +416,15 @@ def main(argv=None):
     ap.add_argument("--device", type=int, default=0)
     ap.add_argument("-S", dest="grab", choices=["all"], help="signal grabber: write every frame's IQ (rtl_433 -S all)")
     ap.add_argument("--grab-dir", default=".", help="directory for the grabbed files (default: the current one)")
+    ap.add_argument("--chunk-mb", type=int, default=0, metavar="N",
+                    help="stream every file through a chain, N MiB of whole blocks per call (bounded host memory)")
     a = ap.parse_args(argv)
-    replay(a.files, a.protocols, a.device, grab_mode=lib.GRAB_ALL if a.grab else 0, grab_dir=a.grab_dir)
+    if a.chunk_mb < 0:
+        ap.error("--chunk-mb must be positive")
+    if a.grab and a.chunk_mb:
+        ap.error("-S does not run with --chunk-mb: the signal grabber does not run on chained batches")
+    replay(a.files, a.protocols, a.device, grab_mode=lib.GRAB_ALL if a.grab else 0, grab_dir=a.grab_dir,
+           chunk_mb=a.chunk_mb)
 
 
 if __name__ == "__main__":

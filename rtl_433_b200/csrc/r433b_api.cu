@@ -127,11 +127,52 @@ struct r433b_ctx {
     uint64_t grab_prior_bytes = 0;    // of which the device copy of the tail holds the last ones
     std::vector<uint64_t> grab_cum;   // run offset of stream i within the batch (used bytes), n_streams + 1
     DevBuf d_grab_prior, d_grab_segs, d_grab_stage;
+    // the last batch was a chained one (r433b_process_chained): absolute sample index of each stream's first sample
+    bool chained = false;
+    std::vector<uint64_t> chain_base;
+    std::vector<r433b_chain *> chains; // alive: r433b_destroy() frees their device memory and detaches them
+};
+
+// What must not change while a chain has an open file: everything the carried state depends on
+struct ChainSettings {
+    uint32_t sample_format, samp_rate, center_frequency, fpdm, block_bytes;
+    int use_mag, enable_fm;
+    float level_limit, min_level, min_snr, fm_low_pass;
+    bool operator==(ChainSettings const &o) const
+    {
+        return sample_format == o.sample_format && samp_rate == o.samp_rate && center_frequency == o.center_frequency
+                && fpdm == o.fpdm && block_bytes == o.block_bytes && use_mag == o.use_mag && enable_fm == o.enable_fm
+                && level_limit == o.level_limit && min_level == o.min_level && min_snr == o.min_snr
+                && fm_low_pass == o.fm_low_pass;
+    }
+};
+
+struct r433b_chain {
+    r433b_ctx *ctx = nullptr;
+    uint32_t n = 0;
+    // device: StreamState per slot, the pulse-train scratch per slot, copies of both taken in front of every batch
+    // (a batch whose result arenas overflow is run again from them), the cont / last flags and the bases of a batch
+    DevBuf d_state, d_train, d_state_copy, d_train_copy, d_flags, d_base;
+    std::vector<uint8_t> open;     // slot i is inside a file
+    std::vector<uint64_t> next;    // ... whose next chunk starts at this absolute sample
+    std::vector<uint64_t> base;    // first sample of slot i's chunk in the last chained batch
+    ChainSettings settings{};
 };
 
 struct r433b_pulses {
     PulseSet set;
 };
+
+namespace {
+void chain_free_device(r433b_chain *ch)
+{
+    for (DevBuf *b : {&ch->d_state, &ch->d_train, &ch->d_state_copy, &ch->d_train_copy, &ch->d_flags, &ch->d_base}) {
+        if (b->p) cudaFree(b->p);
+        b->p = nullptr;
+        b->cap = 0;
+    }
+}
+} // namespace
 
 namespace {
 
@@ -237,6 +278,10 @@ void r433b_destroy(r433b_ctx *ctx)
     if (!ctx) return;
     if (ctx->worker.joinable()) ctx->worker.join();
     cudaSetDevice(ctx->device);
+    for (r433b_chain *ch : ctx->chains) { // a chain outliving its context only holds host memory from here on
+        chain_free_device(ch);
+        ch->ctx = nullptr;
+    }
     for (DevBuf *b : {&ctx->d_data, &ctx->d_offsets, &ctx->d_train, &ctx->d_pkgs, &ctx->d_ppool, &ctx->d_gpool,
                  &ctx->d_counters, &ctx->d_am, &ctx->d_fm, &ctx->d_devparams, &ctx->d_lists, &ctx->d_pairs,
                  &ctx->d_arena, &ctx->d_cursor, &ctx->d_ranges, &ctx->d_state, &ctx->d_lengths, &ctx->d_stage, &ctx->d_raw, &ctx->d_log, &ctx->d_amoff, &ctx->d_chunks, &ctx->d_tiles,
@@ -427,9 +472,8 @@ int slice_ranges(r433b_ctx *ctx, std::vector<GroupRange> const &ranges, unsigned
     return R433B_OK;
 }
 
-} // namespace
-
-int r433b_process(r433b_ctx *ctx, r433b_batch const *b)
+// rtl_433 -r on every stream of the batch; with a chain, stream i is the next chunk of slot i's file (r433b.h)
+int process_iq(r433b_ctx *ctx, r433b_batch const *b, r433b_chain *ch, uint8_t const *last)
 {
     if (!ctx || !b || !b->offsets || (b->n_streams && !b->data)) return fail(ctx, R433B_EINVAL, "null argument");
     if (b->sample_format != R433B_FMT_CU8 && b->sample_format != R433B_FMT_CS16 && b->sample_format != R433B_FMT_CS8
@@ -448,8 +492,30 @@ int r433b_process(r433b_ctx *ctx, r433b_batch const *b)
         if (b->offsets[i] % (16 * in_div)) return fail(ctx, R433B_EINVAL, "stream offsets must be multiples of 16 bytes (32 for cf32)");
         if (i && b->offsets[i] < b->offsets[i - 1]) return fail(ctx, R433B_EINVAL, "offsets not ascending");
     }
+    int enable_fm = 0;
+    for (auto const &d : ctx->devs)
+        if (d.modulation >= 16) enable_fm = 1;
+    // src/rtl_433.c:1094-1102 and :1515-1522
+    unsigned const fpdm = b->fpdm_mode == R433B_FPDM_AUTO ? (b->center_frequency > 800000000u ? 1u : 0u) : b->fpdm_mode;
+    ChainSettings const settings{b->sample_format, b->samp_rate, b->center_frequency, fpdm, block_bytes, ctx->use_mag, enable_fm,
+                                 ctx->level_limit, ctx->min_level, ctx->min_snr, ctx->fm_low_pass};
+    if (ch) {
+        if (ch->ctx != ctx || !last) return fail(ctx, R433B_EINVAL, "r433b_process_chained: chain of another context, or no last[]");
+        if (b->n_streams != ch->n) return fail(ctx, R433B_EINVAL, "r433b_process_chained: n_streams differs from the chain's");
+        if (std::find(ch->open.begin(), ch->open.end(), 1) != ch->open.end() && !(settings == ch->settings))
+            return fail(ctx, R433B_ESTATE, "r433b_process_chained: format, rate, frequency, block size, levels or FM "
+                                           "settings changed while a file of the chain is open");
+        // a chunk that the file goes on behind is whole blocks: the next one starts on a block boundary
+        for (uint32_t i = 0; i < b->n_streams; ++i) {
+            uint64_t const in_bytes = b->lengths ? b->lengths[i] : b->offsets[i + 1] - b->offsets[i];
+            if (!last[i] && in_bytes % ((uint64_t)block_bytes * in_div))
+                return fail(ctx, R433B_EINVAL, "r433b_process_chained: a chunk that is not its file's last must be whole "
+                                               "blocks (block_bytes, 2 x block_bytes of cf32 input)");
+        }
+    }
     CU(cudaSetDevice(ctx->device));
     ctx->processed = ctx->fetched = false;
+    ctx->chained = false;
     ctx->pulse_mode = false;
     ctx->batch = *b;
     ctx->batch.sample_format = (uint32_t)SS; // the host replay only needs the sample size (dm_state.sample_size)
@@ -473,11 +539,8 @@ int r433b_process(r433b_ctx *ctx, r433b_batch const *b)
     for (uint64_t v : ctx->lengths) used_bytes += v;
     uint32_t const n_devs = (uint32_t)ctx->devs.size();
 
-    // src/rtl_433.c:1094-1102 and :1515-1522
-    ctx->fpdm = b->fpdm_mode == R433B_FPDM_AUTO ? (b->center_frequency > 800000000u ? 1u : 0u) : b->fpdm_mode;
-    ctx->enable_fm = 0;
-    for (auto const &d : ctx->devs)
-        if (d.modulation >= 16) ctx->enable_fm = 1;
+    ctx->fpdm = fpdm;
+    ctx->enable_fm = enable_fm;
 
     cudaStream_t const st = 0;
     ctx->d2h_done = false;
@@ -553,6 +616,47 @@ int r433b_process(r433b_ctx *ctx, r433b_batch const *b)
     dp.tile_info = (TileInfo const *)ctx->d_tiles.p;
     dp.fm_out = b->want_stages ? (int16_t *)ctx->d_fm.p : nullptr;
 
+    // a chained batch: the chain's state and pulse trains, which slots continue a file, which files end, where each
+    // chunk lies in its file.  The state is copied first, so that a run that has to be repeated starts from it again.
+    std::vector<uint64_t> base;
+    if (ch && b->n_streams) {
+        size_t const n = b->n_streams;
+        std::vector<uint8_t> flags(2 * n);
+        base.resize(n);
+        for (size_t i = 0; i < n; ++i) {
+            flags[i] = ch->open[i];
+            flags[n + i] = last[i] ? 1 : 0;
+            base[i] = ch->open[i] ? ch->next[i] : 0;
+        }
+        CU(cudaMemcpy(ch->d_flags.p, flags.data(), 2 * n, cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(ch->d_base.p, base.data(), n * sizeof(uint64_t), cudaMemcpyHostToDevice));
+        CU(cudaMemcpyAsync(ch->d_state_copy.p, ch->d_state.p, n * sizeof(StreamState), cudaMemcpyDeviceToDevice, st));
+        CU(cudaMemcpyAsync(ch->d_train_copy.p, ch->d_train.p, n * kTrainInts * sizeof(int), cudaMemcpyDeviceToDevice, st));
+        dp.state = (StreamState *)ch->d_state.p;
+        dp.cont = (unsigned char const *)ch->d_flags.p;
+        dp.last = (unsigned char const *)ch->d_flags.p + n;
+        dp.base = (unsigned long long const *)ch->d_base.p;
+        dp.train_scratch = (int *)ch->d_train.p;
+    }
+    bool detect_ran = false; // a chained batch that runs again restores the chain's state first
+    auto restore_chain = [&]() -> int {
+        if (!ch || !detect_ran || !b->n_streams) return R433B_OK;
+        CU(cudaMemcpyAsync(ch->d_state.p, ch->d_state_copy.p, b->n_streams * sizeof(StreamState), cudaMemcpyDeviceToDevice, st));
+        CU(cudaMemcpyAsync(ch->d_train.p, ch->d_train_copy.p, b->n_streams * kTrainInts * sizeof(int), cudaMemcpyDeviceToDevice, st));
+        return R433B_OK;
+    };
+    auto finish_chain = [&]() {
+        if (!ch) return;
+        for (uint32_t i = 0; i < b->n_streams; ++i) {
+            ch->open[i] = last[i] ? 0 : 1;
+            ch->next[i] = last[i] ? 0 : base[i] + ctx->lengths[i] / SS;
+        }
+        ch->base = base;
+        ch->settings = settings;
+        ctx->chained = true;
+        ctx->chain_base = base;
+    };
+
     uint64_t max_samples = 0;
     for (uint32_t i = 0; i < b->n_streams; ++i) max_samples = std::max<uint64_t>(max_samples, ctx->lengths[i] / SS);
     // k_front over the tiles [sample_begin, sample_end) of every stream, then the walk over the same range
@@ -579,6 +683,8 @@ int r433b_process(r433b_ctx *ctx, r433b_batch const *b)
             fp.tile_info = (TileInfo *)ctx->d_tiles.p;
             fp.counters = q.counters;
             fp.spoil = ctx->spoil_front;
+            fp.state = q.state;
+            fp.cont = q.first_chunk ? q.cont : nullptr;
             uint64_t const warps = (uint64_t)q.n_streams * fp.tiles;
             unsigned const fgrid = (unsigned)((warps + kFrontWarps - 1) / kFrontWarps);
             void (*ffn)(FrontParams) = SS == 2 ? k_front<2> : k_front<4>;
@@ -648,7 +754,8 @@ int r433b_process(r433b_ctx *ctx, r433b_batch const *b)
         dp.pulse_pool = (int *)ctx->d_ppool.p;
         dp.gap_pool = (int *)ctx->d_gpool.p;
         dp.pool_cap = (unsigned)std::min<size_t>(ctx->pool_cap, 0xffffffffu);
-        dp.state = (StreamState *)ctx->d_state.p;
+        if (!ch) dp.state = (StreamState *)ctx->d_state.p;
+        detect_ran = true;
         GroupRange *d_rg = (GroupRange *)ctx->d_ranges.p;
         GroupRange *h_rg = (GroupRange *)ctx->h_ranges.p;
         unsigned const *d_cnt = (unsigned const *)ctx->d_counters.p;
@@ -741,12 +848,14 @@ int r433b_process(r433b_ctx *ctx, r433b_batch const *b)
             }
             ctx->timing.front_ms = frt;
             ctx->timing.front_launches = (unsigned)G;
-            unsigned stat[8];
+            unsigned stat[10];
             CU(cudaMemcpy(stat, ctx->d_counters.p, sizeof(stat), cudaMemcpyDeviceToHost));
             ctx->timing.front_redone = stat[4];
             ctx->timing.front_repairs = stat[5];
             ctx->timing.idle_skipped = stat[6];
             ctx->timing.idle_rewalks = stat[7];
+            ctx->timing.chain_folds = stat[8];
+            ctx->timing.chain_fm_rebuilds = stat[9];
             ctx->timing.h2d_ms = 0; // overlapped: only the wall total is meaningful
             ctx->timing.d2h_ms = 0;
             ctx->timing.detect_ms = det;
@@ -755,6 +864,7 @@ int r433b_process(r433b_ctx *ctx, r433b_batch const *b)
             ctx->timing.detect_launches = (unsigned)G;
             ctx->timing.slice_launches = (unsigned)G;
             ctx->processed = true;
+            finish_chain();
             return R433B_OK;
         }
         // an arena was too small: grow from what the device counted and redo sequentially below
@@ -783,8 +893,9 @@ int r433b_process(r433b_ctx *ctx, r433b_batch const *b)
     CU(cudaEventRecord(ctx->ev[1], st));
 
     unsigned detect_launches = 0;
-    unsigned counters[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    unsigned counters[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
     for (int attempt = 0; attempt < 3; ++attempt) {
+        if (int r = restore_chain()) return r;
         if (int r = dev_reserve(ctx, ctx->d_pkgs, ctx->pkg_cap * sizeof(r433b_package))) return r;
         if (int r = dev_reserve(ctx, ctx->d_ppool, ctx->pool_cap * sizeof(int))) return r;
         if (int r = dev_reserve(ctx, ctx->d_gpool, ctx->pool_cap * sizeof(int))) return r;
@@ -798,6 +909,7 @@ int r433b_process(r433b_ctx *ctx, r433b_batch const *b)
             launch_detect(dp, st, ctx->ev[4]);
             CU(cudaGetLastError());
             detect_launches++;
+            detect_ran = true;
         }
         CU(cudaMemcpyAsync(counters, ctx->d_counters.p, sizeof(counters), cudaMemcpyDeviceToHost, st));
         CU(cudaStreamSynchronize(st));
@@ -827,10 +939,65 @@ int r433b_process(r433b_ctx *ctx, r433b_batch const *b)
     ctx->timing.front_repairs = counters[5];
     ctx->timing.idle_skipped = counters[6];
     ctx->timing.idle_rewalks = counters[7];
+    ctx->timing.chain_folds = counters[8];
+    ctx->timing.chain_fm_rebuilds = counters[9];
     cudaEventElapsedTime(&ctx->timing.total_ms, ctx->ev[0], ctx->ev[3]);
     ctx->timing.d2h_ms = 0;
     ctx->timing.detect_launches = detect_launches;
     ctx->processed = true;
+    finish_chain();
+    return R433B_OK;
+}
+
+} // namespace
+
+int r433b_process(r433b_ctx *ctx, r433b_batch const *b) { return process_iq(ctx, b, nullptr, nullptr); }
+
+int r433b_chain_create(r433b_ctx *ctx, uint32_t n_streams, r433b_chain **out)
+{
+    if (!ctx || !out || !n_streams) return fail(ctx, R433B_EINVAL, "r433b_chain_create: null argument or no streams");
+    *out = nullptr;
+    CU(cudaSetDevice(ctx->device));
+    r433b_chain *ch = new (std::nothrow) r433b_chain();
+    if (!ch) return R433B_ENOMEM;
+    ch->ctx = ctx;
+    ctx->chains.push_back(ch);
+    ch->n = n_streams;
+    ch->open.assign(n_streams, 0);
+    ch->next.assign(n_streams, 0);
+    size_t const n = n_streams;
+    for (auto [buf, bytes] : {std::pair<DevBuf *, size_t>{&ch->d_state, n * sizeof(StreamState)}, {&ch->d_state_copy, n * sizeof(StreamState)},
+                              {&ch->d_train, n * kTrainInts * sizeof(int)}, {&ch->d_train_copy, n * kTrainInts * sizeof(int)},
+                              {&ch->d_flags, 2 * n}, {&ch->d_base, n * sizeof(uint64_t)}})
+        if (int r = dev_reserve(ctx, *buf, bytes)) {
+            r433b_chain_destroy(ch);
+            return r;
+        }
+    *out = ch;
+    return R433B_OK;
+}
+
+void r433b_chain_destroy(r433b_chain *ch)
+{
+    if (!ch) return;
+    if (r433b_ctx *ctx = ch->ctx) {
+        ctx->chains.erase(std::remove(ctx->chains.begin(), ctx->chains.end(), ch), ctx->chains.end());
+        cudaSetDevice(ctx->device);
+        chain_free_device(ch);
+    }
+    delete ch;
+}
+
+int r433b_process_chained(r433b_ctx *ctx, r433b_batch const *b, r433b_chain *chain, uint8_t const *last)
+{
+    if (!chain || !chain->ctx) return fail(ctx, R433B_EINVAL, "r433b_process_chained: no chain, or its context is gone");
+    return process_iq(ctx, b, chain, last);
+}
+
+int r433b_chain_base(r433b_chain const *chain, uint32_t stream, uint64_t *first_sample)
+{
+    if (!chain || !first_sample || stream >= chain->n) return R433B_EINVAL;
+    *first_sample = stream < chain->base.size() ? chain->base[stream] : 0;
     return R433B_OK;
 }
 
@@ -944,7 +1111,8 @@ float r433b_package_file_pos(r433b_ctx const *ctx, r433b_results const *res, uin
     if (ctx->pulse_mode) return 0.0f; // demod->sample_file_pos = 0.0 in front of the .ook loop, src/rtl_433.c:1752
     r433b_package const &k = res->packages[package];
     uint64_t SS = ctx->batch.sample_format;
-    uint64_t bytes = ctx->lengths[k.stream];
+    // a chained chunk: the bytes of its file up to the chunk's end (k.block is absolute)
+    uint64_t bytes = ctx->lengths[k.stream] + (ctx->chained ? ctx->chain_base[k.stream] * SS : 0);
     uint32_t bb = ctx->batch.block_bytes;
     uint64_t n_blocks = (bytes + bb - 1) / bb;
     if (n_blocks == 0) return 0.0f;
@@ -1604,6 +1772,9 @@ int r433b_grab_plan(r433b_ctx *ctx, r433b_results const *res, int mode, r433b_gr
         if (prior && prior->pushed && !prior->tail) return fail(ctx, R433B_EINVAL, "prior ring without its tail");
         if (!ctx->fetched) return fail(ctx, R433B_ESTATE, "r433b_grab_plan before r433b_fetch");
         if (ctx->pulse_mode) return fail(ctx, R433B_ESTATE, "a batch of loaded pulse data has no IQ to grab");
+        if (ctx->chained)
+            return fail(ctx, R433B_ESTATE, "the grabber does not run on chained batches: the reference has no ring order "
+                                           "for files that are open at the same time");
         if (res->packages != (r433b_package const *)ctx->h_pkgs.p || res->n_packages != ctx->n_pkgs)
             return fail(ctx, R433B_EINVAL, "results are not the context's last fetched batch");
         if (mode != R433B_GRAB_ALL)

@@ -71,12 +71,8 @@ struct FmJob {
     int fm_on;                 // 0: "FM" is the raw envelope (buf.fm aliases buf.temp when nothing asks for FM)
     int use_mag;
     int monotone;              // the state rebuild by range collapse is valid
-};
-
-// The exact FM filter state (y, xf) after sample pos - 1
-struct FmState {
-    unsigned long long pos;
-    int y, xf;
+    FmState start;             // the exact state in front of sample 0 (reset state, or carried into a chained chunk)
+    int pri0, prq0;            // the IQ sample in front of sample 0 (centred; zero at a file start)
 };
 
 // Warp-uniform state of the walk.  It lives in shared memory BETWEEN the phases of the walk (idle_run, burst_run,
@@ -102,6 +98,7 @@ struct WalkConst {
     Levels lv;
     int per_ms, fpdm, defer_f1;
     unsigned stream, block_samples;
+    unsigned long long base;     // absolute sample index of sample 0 (chained chunks): added to reported positions
     r433b_package *pkgs;
     int *pulse_pool, *gap_pool;
     unsigned pkg_cap, pool_cap;
@@ -124,16 +121,6 @@ struct alignas(16) WarpSmem {
     WalkConst wc;
 };
 
-// Everything one stream carries from one launch to the next when a batch is processed in time slices.
-struct StreamState {
-    DetState d;
-    int y_am;
-    FmState fm_state;
-    unsigned log_n, last_start, last_count;
-    unsigned seq;
-    int flushed;
-};
-
 struct DetectParams {
     uint8_t const *data;
     unsigned long long const *offsets; // bytes, n_streams + 1
@@ -142,8 +129,12 @@ struct DetectParams {
     unsigned n_streams;
     unsigned stream0, stream_end;      // the streams this launch covers
     unsigned long long sample_begin, sample_end; // the slice of every stream this launch covers (multiples of the tile)
-    int first_chunk;                   // start from reset_sdr_flow() state instead of the saved one
-    struct StreamState *state;         // per-stream carried state between launches of one batch
+    int first_chunk;                   // the first launch of the batch: start from reset_sdr_flow() state instead of the
+                                       // saved one, except for the streams `cont` marks
+    struct StreamState *state;         // per-stream carried state between launches (and chained batches)
+    unsigned char const *cont;         // chained: 1 = the stream continues a file, its first launch loads state[s]
+    unsigned char const *last;         // chained: 1 = the file ends with this chunk (flush); nullptr: every file ends
+    unsigned long long const *base;    // chained: absolute sample index of each stream's sample 0 (nullptr: 0)
     int use_mag, enable_fm, fpdm;
     unsigned flip; // XOR mask applied to every loaded word: 0x80808080 turns cs8 into cu8
     unsigned rate, block_samples;
@@ -205,18 +196,10 @@ __device__ R4_NOINLINE void disc_fill(FmJob const &jb, WarpSmem &sm, unsigned lo
 {
     constexpr int SPL = 16 / SS;
     int const lane = threadIdx.x & 31;
-    int pri = 0, prq = 0; // IQ in front of the batch (zero in front of the stream: reset demod state)
-    if (jb.fm_on && a > 0) {
-        uint8_t const *g = jb.src + (a - 1) * SS;
-        if (SS == 2) {
-            pri = (int)(g[0] ^ (jb.flip & 0xff)) - 128;
-            prq = (int)(g[1] ^ (jb.flip & 0xff)) - 128;
-        } else {
-            uint32_t w = *reinterpret_cast<uint32_t const *>(g) ^ jb.flip;
-            pri = (int)(int16_t)(w & 0xffff);
-            prq = (int)(int16_t)(w >> 16);
-        }
-    }
+    R4_EMU_ASSERT_POS(a);
+    // IQ in front of the batch: at sample 0 the one carried into the chunk (zero at a file start: reset demod state)
+    int pri = jb.pri0, prq = jb.prq0;
+    if (jb.fm_on && a > 0) iq_at<SS>(jb.src, a - 1, jb.flip, pri, prq);
 #pragma unroll 1
     for (int base = 0; base < n; base += 32 * SPL) {
         int const i0 = base + lane * SPL;
@@ -262,7 +245,7 @@ __device__ R4_NOINLINE void disc_fill(FmJob const &jb, WarpSmem &sm, unsigned lo
 // The exact FM filter state in front of sample `pos` (after sample pos - 1), without knowing anything
 // before: both ends of the state range go through the K samples in front of pos; when they meet, the value
 // is independent of everything earlier.  K grows until they meet or the walk starts at a known state
-// (the stream start, or sm.fm_state.pos).  Monotone filters only.  Leaves the state in sm.fm_state.
+// (sample 0, where jb.start holds it, or sm.fm_state.pos).  Monotone filters only.  Leaves the state in sm.fm_state.
 template <int SS>
 __device__ R4_NOINLINE void fm_cold(FmJob const &jb, WarpSmem &sm, unsigned long long pos)
 {
@@ -278,8 +261,8 @@ __device__ R4_NOINLINE void fm_cold(FmJob const &jb, WarpSmem &sm, unsigned long
             exact_start = true;
         }
         if (exact_start) {
-            lo = hi = a == known ? sm.fm_state.y : 0;
-            fp = a == known ? sm.fm_state.xf : 0;
+            lo = hi = a == known ? sm.fm_state.y : jb.start.y;
+            fp = a == known ? sm.fm_state.xf : jb.start.xf;
         } else {
             lo = SS == 2 ? -32768 : (int)0x80000000;
             hi = SS == 2 ? 32767 : 0x7fffffff;
@@ -473,6 +456,7 @@ __device__ R4_NOINLINE int f1_evaluate(FmJob const &jb, WarpSmem &sm, unsigned c
             unsigned st, cnt;
             entry(j, st, cnt);
             unsigned long long pos = start_abs + st;
+            R4_EMU_ASSERT_POS(pos); // a chunk end folds the log: no entry points in front of the chunk
             while (cnt) {
                 fm_cover<SS>(jb, sm, pos);
                 unsigned long long wend = sm.win0 + (unsigned long long)sm.win_n;
@@ -631,6 +615,8 @@ __device__ R4_NOINLINE void walk_emit(WarpSmem &sm, int type, unsigned long long
             wc.gap_pool[off + i] = sg[i];
         }
         if (lane == 0) {
+            // positions inside the chunk; a chunk is whole blocks, so the block phase is the absolute one and the
+            // differences (start_ago: start_abs may lie in front of the chunk, wrapped) are those of the whole file
             unsigned long long blk = flush ? (N + wc.block_samples - 1) / wc.block_samples : pos / wc.block_samples;
             unsigned long long bstart = blk * wc.block_samples;
             unsigned long long blen = flush ? 0 : (N - bstart < wc.block_samples ? N - bstart : wc.block_samples);
@@ -638,9 +624,9 @@ __device__ R4_NOINLINE void walk_emit(WarpSmem &sm, int type, unsigned long long
             k.stream = wc.stream;
             k.seq = seq;
             k.type = type;
-            k.block = (int)blk;
-            k.offset = h.offset;
-            k.end_pos = pos;
+            k.block = (int)(blk + wc.base / wc.block_samples);
+            k.offset = h.offset + wc.base;
+            k.end_pos = pos + wc.base;
             k.start_ago = flush ? (unsigned)(N - h.start_abs) : (unsigned)(bstart + blen - h.start_abs);
             k.end_ago = flush ? 0u : (unsigned)(blen - (pos - bstart));
             k.num_pulses = h.num_pulses;
@@ -1329,6 +1315,49 @@ __device__ R4_NOINLINE int generic_step(WarpSmem &sm, int n)
     return n + adv;
 }
 
+// The end of a chunk of a file that goes on in the next chained batch (the launch that reaches it has walked its last
+// tile: idle_skip never skips the last tile of a range).  Nothing the next chunk reads may lie in front of it: the
+// deferred carrier-estimate log is folded into its exact value, the FM filter state is made exact at the chunk end (a
+// monotone filter by range collapse, which reaches back no further than the state known in this chunk; any other
+// forward from the last exact state), and the chunk's last IQ sample is kept.  Positions are rebased to the next
+// chunk's sample 0.  `ss` receives what the next chunk starts from.
+template <int SS>
+__device__ R4_NOINLINE void chunk_end(WarpSmem &sm, StreamState *ss)
+{
+    int const lane = threadIdx.x & 31;
+    __syncwarp();
+    FmJob const &jb = sm.wc.jb;
+    unsigned long long const N = jb.N;
+    if (sm.ws.log_n || sm.ws.log_count) {
+        walk_f1_fold<SS>(sm);
+        if (lane == 0) atomicAdd(&sm.wc.counters[8], 1u);
+    }
+    if (jb.fm_on && sm.fm_state.pos != N) {
+        if (jb.monotone) {
+            fm_cold<SS>(jb, sm, N);
+        } else {
+            while (sm.fm_state.pos < N) {
+                unsigned long long const w0 = sm.fm_state.pos;
+                fm_window<SS>(jb, sm, w0, N - w0 < (unsigned long long)kFmWin ? (int)(N - w0) : kFmWin);
+            }
+        }
+        if (lane == 0) atomicAdd(&sm.wc.counters[9], 1u);
+    }
+    int ci, cq;
+    iq_at<SS>(jb.src, N - 1, jb.flip, ci, cq);
+    __syncwarp();
+    if (lane == 0) {
+        if (!jb.fm_on) sm.fm_state = FmState{N, 0, 0}; // unused: "FM" is the raw envelope
+        sm.fm_state.pos -= N;
+        sm.ws.d.start_abs -= N;
+        sm.ws.d.fsk_offset -= N;
+        ss->fm_start = sm.fm_state;
+        ss->iq_i = ci;
+        ss->iq_q = cq;
+    }
+    __syncwarp();
+}
+
 // --------------------------------------------------------------------------- kernel ------
 
 template <int SS>
@@ -1356,6 +1385,8 @@ __global__ void __launch_bounds__(kDetectWarps * 32, kDetectCtasPerSm) k_detect(
 
     int y_am = 0; // the last AM value of the previous tile: the AM filter state (reset_sdr_flow(): zero)
     int flushed = 0;
+    // a stream that continues a file (chained batch) loads its state in the batch's first launch too
+    bool const fresh = p.first_chunk && !(p.cont && p.cont[s]);
     if (lane == 0) {
         WalkConst &wc = sm.wc;
         wc.jb.src = src;
@@ -1378,6 +1409,7 @@ __global__ void __launch_bounds__(kDetectWarps * 32, kDetectCtasPerSm) k_detect(
         wc.defer_f1 = defer_f1;
         wc.stream = s;
         wc.block_samples = p.block_samples;
+        wc.base = p.base ? p.base[s] : 0;
         wc.pkgs = p.pkgs;
         wc.pulse_pool = p.pulse_pool;
         wc.gap_pool = p.gap_pool;
@@ -1392,12 +1424,18 @@ __global__ void __launch_bounds__(kDetectWarps * 32, kDetectCtasPerSm) k_detect(
         ws.nv_tile = 0;
         ws.skip_y = 0;
         ws.rewalk_end = 0;
-        if (p.first_chunk) {
+        if (fresh) {
             det_reset(ws.d);
             ws.d.ook_hw = ws.d.fsk_hw = kMaxPulses; // scratch is not assumed to be zero: first package clears it
             ws.log_n = ws.log_start = ws.log_count = 0;
             ws.seq = 0;
             sm.fm_state = FmState{0, 0, 0};
+            wc.jb.start = FmState{0, 0, 0};
+            wc.jb.pri0 = wc.jb.prq0 = 0;
+            if (p.state) {
+                p.state[s].fm_start = wc.jb.start;
+                p.state[s].iq_i = p.state[s].iq_q = 0;
+            }
         } else {
             StreamState const &ss = p.state[s];
             ws.d = ss.d;
@@ -1406,14 +1444,15 @@ __global__ void __launch_bounds__(kDetectWarps * 32, kDetectCtasPerSm) k_detect(
             ws.log_start = ss.last_start;
             ws.log_count = ss.last_count;
             sm.fm_state = ss.fm_state;
+            wc.jb.start = ss.fm_start;
+            wc.jb.pri0 = ss.iq_i;
+            wc.jb.prq0 = ss.iq_q;
         }
         sm.win0 = 0;
         sm.win_n = 0;
     }
-    if (!p.first_chunk) {
-        y_am = p.state[s].y_am;
-        flushed = p.state[s].flushed;
-    }
+    if (!fresh) y_am = p.state[s].y_am;
+    if (!p.first_chunk) flushed = p.state[s].flushed;
     __syncwarp();
 
     int const a1 = p.lpf_a1, b0 = p.lpf_b0;
@@ -1437,10 +1476,13 @@ __global__ void __launch_bounds__(kDetectWarps * 32, kDetectCtasPerSm) k_detect(
 #pragma unroll
             for (int i = 0; i < 8; ++i) v[i] = g[i];
             ChunkInfo const ci = chunk_stream[t0 / C + lane];
+            // the first tile of a stream starts from the reset state in k_front, the first of a continued chunk from the
+            // carried state (exact as well, but checked: it is the tile a spoiled guess of the tests lands on)
+            bool const handover = t0 != 0 || (p.cont && p.cont[s]); // t0 == 0: read here, not kept live across the walk
             int x0 = 0, xm = 0;
-            if (t0 != 0) {
+            if (handover) {
                 x0 = env_at<SS>(src, t0, p.flip, p.use_mag);
-                xm = env_at<SS>(src, t0 - 1, p.flip, p.use_mag);
+                xm = t0 != 0 ? env_at<SS>(src, t0 - 1, p.flip, p.use_mag) : env_iq<SS>(sm.wc.jb.pri0, sm.wc.jb.prq0, p.use_mag);
             }
 #ifndef R433B_SIMT_EMU
             if (t0 + T < N) {
@@ -1467,8 +1509,8 @@ __global__ void __launch_bounds__(kDetectWarps * 32, kDetectCtasPerSm) k_detect(
                 sm.ws.nv_tile = nv_tile;
             }
             __syncwarp();
-            // hand-over check (see the file header): the first tile of a stream starts from the reset state in k_front
-            if (t0 != 0) {
+            // hand-over check (see the file header)
+            if (handover) {
                 // the reference keeps x[-1] as int16 across block calls (src/baseband.c:167)
                 if (t0 % p.block_samples == 0) xm = (int)(int16_t)xm;
                 int const expect = iir16_nowrap(y_am, a1, b0, x0 + xm);
@@ -1501,7 +1543,12 @@ __global__ void __launch_bounds__(kDetectWarps * 32, kDetectCtasPerSm) k_detect(
         __syncwarp();
     }
 
-    // flush_sdr_flow(): len == 0 call(s) at the end of the file, in the launch that reaches it
+    // flush_sdr_flow(): len == 0 call(s) at the end of the file, in the launch that reaches it; the end of a chunk of a
+    // file that goes on hands its state to the next chunk instead
+    if (N <= p.sample_end && !flushed && p.last && !p.last[s]) {
+        if (N) chunk_end<SS>(sm, p.state + s);
+        flushed = 1;
+    }
     if (N <= p.sample_end && !flushed) {
         for (;;) {
             __syncwarp();
@@ -1529,11 +1576,12 @@ __global__ void __launch_bounds__(kDetectWarps * 32, kDetectCtasPerSm) k_detect(
     }
 
     // ---- stage dump: FM (the raw envelope with FM off) of every sample, after the walk and apart from it ----------
-    // From the reset state over [0, N): the host gives a batch with stage arrays one launch over whole streams.
+    // From the state in front of sample 0 over [0, N): the host gives a batch with stage arrays one launch over whole
+    // streams (chunks).
     if (p.fm_out) {
         if (lane == 0) {
             sm.wc.jb.fm_out = p.fm_out + byte0 / SS; // the walk is over: its job can take the dump
-            sm.fm_state = FmState{0, 0, 0};
+            sm.fm_state = sm.wc.jb.start;
         }
         __syncwarp();
         for (unsigned long long w0 = 0; w0 < N; w0 += kFmWin)

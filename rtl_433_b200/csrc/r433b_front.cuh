@@ -26,9 +26,12 @@
 #ifdef R433B_SIMT_EMU
 #define R4_DYN_SMEM(type, name) type *name = reinterpret_cast<type *>(simt::st().dyn_smem)
 #define R4_NOINLINE
+// a chained chunk has no samples in front of its start: no stream index may go below 0
+#define R4_EMU_ASSERT_POS(pos) assert((long long)(pos) >= 0)
 #else
 #define R4_DYN_SMEM(type, name) extern __shared__ __align__(16) type name[]
 #define R4_NOINLINE __noinline__
+#define R4_EMU_ASSERT_POS(pos) ((void)0)
 #endif
 
 namespace r433b {
@@ -57,6 +60,26 @@ struct alignas(16) TileInfo {
     int32_t pad;
 };
 
+// The exact FM filter state (y, xf) after sample pos - 1
+struct FmState {
+    unsigned long long pos;
+    int y, xf;
+};
+
+// Everything one stream carries from one launch to the next: between the time slices of a batch, and between the
+// chunks of a chained batch (r433b_process_chained), where a chunk ends on a block boundary and the next one starts
+// its positions at 0 again (start_abs, fsk_offset and fm_state.pos are rebased by the chunk's length).
+struct StreamState {
+    DetState d;
+    int y_am;
+    FmState fm_state;
+    unsigned log_n, last_start, last_count;
+    unsigned seq;
+    int flushed;      // the end of the stream's range (flush, or the end of a chunk of a file that goes on) is done
+    FmState fm_start; // in front of the chunk: the FM filter state (pos 0) ...
+    int iq_i, iq_q;   // ... and the last IQ sample of the previous chunk (centred); zero at a file start
+};
+
 // 16 contiguous bytes (8 cu8 / 4 cs16 samples) starting at sample `pos` of the stream: one 128-bit load;
 // zero-filled past `n_valid` samples counted from pos.
 template <int SS>
@@ -64,6 +87,7 @@ __device__ __forceinline__ void load_group(uint8_t const *src, unsigned long lon
         uint32_t (&rw)[4])
 {
     constexpr int SPL = 16 / SS;
+    R4_EMU_ASSERT_POS(pos);
     uint8_t const *g = src + pos * SS;
     if (n_valid >= SPL) {
         uint4 v = __ldg(reinterpret_cast<uint4 const *>(g));
@@ -131,6 +155,7 @@ __device__ __forceinline__ void env_group(uint32_t const (&rw)[4], int use_mag, 
 template <int SS>
 __device__ __forceinline__ int env_at(uint8_t const *src, unsigned long long pos, unsigned flip, int use_mag)
 {
+    R4_EMU_ASSERT_POS(pos);
     uint8_t const *g = src + pos * SS;
     if (SS == 2) {
         unsigned const w = (unsigned)*reinterpret_cast<uint16_t const *>(g) ^ (flip & 0xffff); // streams start 16-byte aligned
@@ -139,6 +164,30 @@ __device__ __forceinline__ int env_at(uint8_t const *src, unsigned long long pos
     }
     uint32_t w = *reinterpret_cast<uint32_t const *>(g) ^ flip;
     return mag_cs16((int)(int16_t)(w & 0xffff), (int)(int16_t)(w >> 16));
+}
+
+// envelope / magnitude of a centred IQ sample (StreamState::iq_i / iq_q: the sample in front of a chained chunk)
+template <int SS>
+__device__ __forceinline__ int env_iq(int ci, int cq, int use_mag)
+{
+    if (SS == 2) return use_mag ? mag_cu8(ci + 128, cq + 128) : env_cu8(ci + 128, cq + 128);
+    return mag_cs16(ci, cq);
+}
+
+// the centred IQ sample at `pos` (flip applied: cs8 reads as cu8)
+template <int SS>
+__device__ __forceinline__ void iq_at(uint8_t const *src, unsigned long long pos, unsigned flip, int &ci, int &cq)
+{
+    R4_EMU_ASSERT_POS(pos);
+    uint8_t const *g = src + pos * SS;
+    if (SS == 2) {
+        ci = (int)(g[0] ^ (flip & 0xff)) - 128;
+        cq = (int)(g[1] ^ (flip & 0xff)) - 128;
+    } else {
+        uint32_t w = *reinterpret_cast<uint32_t const *>(g) ^ flip;
+        ci = (int)(int16_t)(w & 0xffff);
+        cq = (int)(int16_t)(w >> 16);
+    }
 }
 
 struct FrontParams {
@@ -158,7 +207,10 @@ struct FrontParams {
     TileInfo *tile_info;                  // one per tile of `am`
     unsigned *counters;                   // [4] chunks done twice
     int spoil;                            // tests: 1 = lane 0's guess is made wrong, 2 = every lane's, 3 = lane 0's in every
-                                          // 7th tile (R433B_SPOIL_FRONT)
+                                          // 7th tile, 4 = lane 0's in every tile incl. tile 0 of a continued chunk
+                                          // (R433B_SPOIL_FRONT)
+    StreamState const *state;             // chained batches: the state carried in front of the chunk ...
+    unsigned char const *cont;            // ... for the streams whose flag is set (nullptr: none)
 };
 
 // Shared-memory staging of one tile's IQ: the chunks [-kWarmChunks, 32) of the tile, every chunk (C samples)
@@ -245,6 +297,13 @@ __global__ void __launch_bounds__(kFrontWarps * 32, kFrontCtasPerSm) k_front(Fro
     unsigned long long const gpos = t0 + (unsigned long long)base; // first sample of the chunk in the stream
 
     int y = 0, xp = 0;
+    // the first sample of a continued chunk: the exact state the previous chunk ended with, as for a stream's first
+    // tile (x[-1] is narrowed below: a chunk starts a block)
+    bool const carried = gpos == 0 && p.cont && p.cont[s];
+    if (carried) {
+        y = p.state[s].y_am;
+        xp = env_iq<SS>(p.state[s].iq_i, p.state[s].iq_q, p.use_mag);
+    }
     if (gpos != 0 && nv > 0) { // reads the chunk in front of this lane's: before the __syncwarp() below
         uint32_t rw[4];
         int x[SPL];
@@ -287,8 +346,8 @@ __global__ void __launch_bounds__(kFrontWarps * 32, kFrontCtasPerSm) k_front(Fro
     // the reference keeps x[-1] as int16 across block calls (src/baseband.c:167): only the first sample of a
     // block sees the narrowed value, and block starts are tile starts
     if (gpos % p.block_samples == 0) xp = (int)(int16_t)xp;
-    if (p.spoil && gpos != 0
-            && (p.spoil == 2 || (lane == 0 && (p.spoil == 1 || (p.spoil == 3 && t0 / kTile % 7 == 0)))))
+    if (p.spoil && (gpos != 0 || (p.spoil == 4 && carried))
+            && (p.spoil == 2 || (lane == 0 && (p.spoil == 1 || p.spoil == 4 || (p.spoil == 3 && t0 / kTile % 7 == 0)))))
         y = y > 16000 ? y - 999 : y + 999; // tests: force the redo / repair paths
     int const y_b = y, xp_b = xp;
     int y_end = y, cmin = 32767, cmax = 0;

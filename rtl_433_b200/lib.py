@@ -31,7 +31,8 @@ EXPORTS = ["r433b_create", "r433b_destroy", "r433b_last_error", "r433b_set_level
            "r433b_format_ook", "r433b_format_ook_header", "r433b_format_vcd", "r433b_format_vcd_header",
            "r433b_dump_logic_u8", "r433b_set_gates", "r433b_get_gated",
            "r433b_dispatch_r_devices_parallel", "r433b_analyze", "r433b_analysis_get", "r433b_analysis_text",
-           "r433b_analysis_events", "r433b_submit", "r433b_wait", "r433b_grab_plan", "r433b_grab_copy", "r433b_grab_tail"]
+           "r433b_analysis_events", "r433b_submit", "r433b_wait", "r433b_grab_plan", "r433b_grab_copy", "r433b_grab_tail",
+           "r433b_chain_create", "r433b_chain_destroy", "r433b_process_chained", "r433b_chain_base"]
 
 
 def build(force=False, verbose=False):
@@ -111,7 +112,7 @@ class Timing(C.Structure):
                 ("total_ms", C.c_float), ("detect_launches", C.c_uint32), ("slice_launches", C.c_uint32),
                 ("front_ms", C.c_float), ("front_launches", C.c_uint32), ("front_redone", C.c_uint32),
                 ("front_repairs", C.c_uint32), ("idle_skipped", C.c_uint32), ("idle_rewalks", C.c_uint32),
-                ("grab_ms", C.c_float)]
+                ("grab_ms", C.c_float), ("chain_folds", C.c_uint32), ("chain_fm_rebuilds", C.c_uint32)]
 
 
 GRAB_ALL, GRAB_UNKNOWN, GRAB_KNOWN, GRAB_UNDECODED = 1, 2, 3, 4
@@ -165,6 +166,10 @@ def load():
     L.r433b_set_devices.argtypes = [C.c_void_p, C.POINTER(Device), C.c_uint32]
     L.r433b_set_r_devices.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
     L.r433b_process.argtypes = [C.c_void_p, C.POINTER(Batch)]
+    L.r433b_chain_create.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_void_p)]
+    L.r433b_chain_destroy.argtypes = [C.c_void_p]
+    L.r433b_process_chained.argtypes = [C.c_void_p, C.POINTER(Batch), C.c_void_p, C.c_void_p]
+    L.r433b_chain_base.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint64)]
     L.r433b_fetch.argtypes = [C.c_void_p, C.POINTER(Results)]
     L.r433b_get_timing.argtypes = [C.c_void_p, C.POINTER(Timing)]
     L.r433b_get_counts.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
@@ -329,6 +334,41 @@ def dump_logic_u8(pd, length, buf_offset, bits):
     return out
 
 
+class Chain:
+    """Slots that carry each stream's demodulator state from one chained batch to the next (include/r433b.h:
+    r433b_chain).  Pass it to Context.process(..., chain=, last=).  Context.close() closes the context's chains first;
+    `with lib.Chain(ctx, n) as chain:` closes it at the end of the block."""
+
+    def __init__(self, ctx, n_streams):
+        self.L = ctx.L
+        self.ctx = ctx
+        self.n = n_streams
+        h = C.c_void_p()
+        ctx._check(self.L.r433b_chain_create(ctx.h, n_streams, C.byref(h)))
+        self.h = h
+        ctx._chains.append(self)
+
+    def close(self):
+        if self.h:
+            self.L.r433b_chain_destroy(self.h)
+            self.h = None
+            self.ctx._chains.remove(self)
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def base(self, stream):
+        """Absolute sample index of the first sample of slot `stream`'s chunk in the last chained batch."""
+        out = C.c_uint64()
+        rc = self.L.r433b_chain_base(self.h, stream, C.byref(out))
+        if rc:
+            raise R433Error(f"r433b_chain_base: {rc}")
+        return out.value
+
+
 class Context:
     """One GPU context (include/r433b.h: r433b_ctx)."""
 
@@ -341,8 +381,11 @@ class Context:
         self.h = h
         self._keep = None
         self.n_devices = 0
+        self._chains = []
 
     def close(self):
+        for chain in list(self._chains):
+            chain.close()
         if self.h:
             self.L.r433b_destroy(self.h)
             self.h = None
@@ -382,8 +425,9 @@ class Context:
         return int(self.L.r433b_get_gated(self.h))
 
     def process(self, data, offsets, sample_format, samp_rate=250000, center_frequency=433920000, fpdm_mode=FPDM_AUTO,
-                block_bytes=0, data_on_device=False, want_stages=False, lengths=None):
-        """`data`: host numpy array (any dtype, contiguous) or an int device pointer."""
+                block_bytes=0, data_on_device=False, want_stages=False, lengths=None, chain=None, last=None):
+        """`data`: host numpy array (any dtype, contiguous) or an int device pointer.  With a Chain, stream i is the
+        next chunk of slot i's file and `last[i]` says whether the file ends with it (r433b_process_chained)."""
         offs = np.ascontiguousarray(offsets, dtype=np.uint64)
         if isinstance(data, int):
             ptr = data
@@ -395,7 +439,11 @@ class Context:
                   center_frequency, fpdm_mode, block_bytes, int(data_on_device), int(want_stages),
                   None if lens is None else lens.ctypes.data_as(C.POINTER(C.c_uint64)))
         self._keep = (data, offs, lens)
-        self._check(self.L.r433b_process(self.h, C.byref(b)))
+        if chain is None:
+            self._check(self.L.r433b_process(self.h, C.byref(b)))
+            return
+        flags = np.ascontiguousarray(np.ones(len(offs) - 1) if last is None else last, dtype=np.uint8)
+        self._check(self.L.r433b_process_chained(self.h, C.byref(b), chain.h, flags.ctypes.data))
 
     def process_pulses(self, pulses):
         """All slicers on every package of a Pulses set (the slicer stage only); then fetch()/dispatch as usual."""
