@@ -70,6 +70,9 @@ struct r433b_ctx {
     int enable_fm = 0;
     int n_sms = 132;        // cudaDevAttrMultiProcessorCount of `device`
     int spoil_front = 0; // R433B_SPOIL_FRONT=1|2|3: k_front starts from wrong guesses (tests of the redo / repair paths)
+    // R433B_TEST_CAPS=pkg,pool,arena: initial package / pulse-pool / event-arena caps in place of the defaults (0 keeps
+    // a default), so that small inputs take the overflow-and-rerun paths in the tests; growth is unchanged
+    size_t min_caps[3] = {0, 0, 0};
     Levels lv{};
     // device memory (grow only)
     DevBuf d_data, d_offsets, d_train, d_pkgs, d_ppool, d_gpool, d_counters, d_am, d_fm;
@@ -204,7 +207,12 @@ int dev_reserve(r433b_ctx *ctx, DevBuf &b, size_t bytes)
     if (b.p) cudaFree(b.p);
     b.p = nullptr;
     b.cap = 0;
+#ifdef R433B_EXACT_ALLOC // tests under the emulator: a buffer ends where its cap does, so a guard page behind it
+                         // catches a kernel that writes even one word past the cap
+    size_t want = bytes;
+#else
     size_t want = bytes + bytes / 8 + 256;
+#endif
     cudaError_t e = cudaMalloc(&b.p, want);
     if (e != cudaSuccess) return fail(ctx, R433B_ENOMEM, "cudaMalloc", e);
     b.cap = want;
@@ -267,6 +275,11 @@ int r433b_create(int cuda_device, r433b_ctx **out)
     cudaEventCreateWithFlags(&ctx->ev_init, cudaEventDisableTiming);
     ctx->lv = compute_levels(0, 0.0f, -12.1442f, 9.0f);
     if (char const *v = getenv("R433B_SPOIL_FRONT")) ctx->spoil_front = atoi(v);
+    if (char const *v = getenv("R433B_TEST_CAPS")) {
+        unsigned long long c[3] = {0, 0, 0};
+        sscanf(v, "%llu,%llu,%llu", &c[0], &c[1], &c[2]);
+        for (int i = 0; i < 3; ++i) ctx->min_caps[i] = (size_t)c[i];
+    }
     if (cudaDeviceGetAttribute(&ctx->n_sms, cudaDevAttrMultiProcessorCount, cuda_device) != cudaSuccess || ctx->n_sms <= 0)
         ctx->n_sms = 132;
     *out = ctx;
@@ -701,9 +714,12 @@ int process_iq(r433b_ctx *ctx, r433b_batch const *b, r433b_chain *ch, uint8_t co
     // slicer parameters: per device, scaled to this batch's sample rate on the host
     if (int r = upload_slicer_tables(ctx, std::vector<uint32_t>{b->samp_rate}, st)) return r;
 
-    if (ctx->pkg_cap < (size_t)b->n_streams * 16 + 1024) ctx->pkg_cap = (size_t)b->n_streams * 16 + 1024;
-    if (ctx->pool_cap < ctx->pkg_cap * 128) ctx->pool_cap = ctx->pkg_cap * 128;
-    if (ctx->arena_cap < total_bytes / 2 + (1u << 20)) ctx->arena_cap = total_bytes / 2 + (1u << 20);
+    size_t const pkg_min = ctx->min_caps[0] ? ctx->min_caps[0] : (size_t)b->n_streams * 16 + 1024;
+    if (ctx->pkg_cap < pkg_min) ctx->pkg_cap = pkg_min;
+    size_t const pool_min = ctx->min_caps[1] ? ctx->min_caps[1] : ctx->pkg_cap * 128;
+    if (ctx->pool_cap < pool_min) ctx->pool_cap = pool_min;
+    size_t const arena_min = ctx->min_caps[2] ? ctx->min_caps[2] : total_bytes / 2 + (1u << 20);
+    if (ctx->arena_cap < arena_min) ctx->arena_cap = arena_min;
 
 
     // ---- pipelined path: host input cut into G TIME SLICES of every stream; the copy-in of slice
@@ -1490,7 +1506,8 @@ int r433b_process_pulses(r433b_ctx *ctx, r433b_pulses const *ps)
         CU(cudaStreamSynchronize(st));
     }
     if (n && n_devs) {
-        if (ctx->arena_cap < (size_t)(1u << 20)) ctx->arena_cap = 1u << 20;
+        size_t const arena_min = ctx->min_caps[2] ? ctx->min_caps[2] : (size_t)(1u << 20);
+        if (ctx->arena_cap < arena_min) ctx->arena_cap = arena_min;
         if (int r = upload_slicer_tables(ctx, rates, st)) return r;
         if (int r = slice_ranges(ctx, ranges, n, st)) return r;
         ctx->timing.total_ms = ctx->timing.slice_ms;
