@@ -212,7 +212,8 @@ uint64_t r433b_get_gated(r433b_ctx const *ctx);
 int r433b_copy_stage(r433b_ctx *ctx, uint32_t stream, int16_t *am, int16_t *fm, uint64_t max_samples);
 
 /* Position-independent 64-bit checksum (FNV-1a over 32-bit words) of everything a fetched batch holds for one
-   stream: package headers, pulse / gap widths, the event bytes of every (package, device) pair.  Streams that
+   stream: package headers, pulse / gap widths, the events of every (package, device) pair, hashed as if every
+   event were stored in the long form (no one-word rows or events), with that form's byte count.  Streams that
    carry the same samples have equal digests wherever they sit in a batch. */
 int r433b_stream_digest(r433b_ctx *ctx, r433b_results const *res, uint32_t stream, uint64_t *digest);
 

@@ -1250,8 +1250,8 @@ int replay_stream(r433b_ctx *ctx, r433b_results const *res, uint32_t stream, Per
 extern "C" {
 
 // Position-independent checksum of everything the batch holds for one stream: package headers (without the
-// fields that say where in the batch they lie), pulse and gap widths, and the event bytes of every
-// (package, device) pair in device order.  Two streams with the same samples give the same digest wherever
+// fields that say where in the batch they lie), pulse and gap widths, and the events of every
+// (package, device) pair in device order, each in the long form of the wire format (event_long_form).  Two streams with the same samples give the same digest wherever
 // they sit in a batch.
 int r433b_stream_digest(r433b_ctx *ctx, r433b_results const *res, uint32_t stream, uint64_t *digest)
 {
@@ -1268,6 +1268,7 @@ int r433b_stream_digest(r433b_ctx *ctx, r433b_results const *res, uint32_t strea
     };
     r433b_package const *begin = std::lower_bound(res->packages, res->packages + res->n_packages, stream,
             [](r433b_package const &k, uint32_t s) { return k.stream < s; });
+    std::vector<uint32_t> longform;
     for (r433b_package const *k = begin; k != res->packages + res->n_packages && k->stream == stream; ++k) {
         uint32_t const hdr[] = {k->seq, (uint32_t)k->type, (uint32_t)k->block, (uint32_t)k->offset, (uint32_t)(k->offset >> 32),
                                 ctx->pulse_mode ? 0u : (uint32_t)k->end_pos, ctx->pulse_mode ? 0u : (uint32_t)(k->end_pos >> 32), k->start_ago, k->end_ago, k->num_pulses,
@@ -1278,11 +1279,20 @@ int r433b_stream_digest(r433b_ctx *ctx, r433b_results const *res, uint32_t strea
         mix_words(res->gap_pool + k->pulse_off, k->pulse_count);
         for (uint32_t dv = 0; dv < res->n_devices; ++dv) {
             r433b_pair const &pr = res->pairs[(size_t)k->first_pair + dv];
-            mix(pr.bytes);
+            // the events in their long form, so that the digest does not depend on which of them got one-word forms
+            longform.clear();
+            uint32_t const *ev = reinterpret_cast<uint32_t const *>(res->events + pr.offset);
+            for (uint32_t pos = 0, total = pr.bytes / 4; pos < total;) {
+                EventHead const e = event_head(ev[pos]);
+                if (e.len < 1 || pos + e.len > total || event_long_form(ev + pos, e, longform))
+                    return fail(ctx, R433B_EINVAL, "corrupt event stream");
+                pos += e.len;
+            }
+            mix((uint32_t)longform.size() * 4);
             mix(pr.events);
             mix(pr.gated_single);
             mix(pr.gated_multi);
-            if (pr.bytes) mix_words(res->events + pr.offset, pr.bytes / 4);
+            mix_words(longform.data(), longform.size());
         }
     }
     *digest = h;

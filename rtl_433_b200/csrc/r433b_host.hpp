@@ -101,6 +101,52 @@ inline std::vector<unsigned> slice_list(std::vector<r433b_device> const &devs, i
 }
 
 
+// The header of an event of the wire format (r433b_slice.cuh); len = the event's words.
+struct EventHead {
+    uint32_t num_rows, dirty, free_row, len;
+};
+
+inline EventHead event_head(uint32_t h)
+{
+    if ((h & 0xff) == 0xff) return {1, 0, 1, 1}; // one-word event
+    return {h & 0x7f, (h >> 7) & 1, (h >> 8) & 0xff, h >> 16};
+}
+
+// The rows of the event at ev (len words, head e), each as in the long form whatever form it is stored in:
+// row(r, bits, syncs, data, words) with `words` data words at `data`.  Returns the offset of the first word after the
+// rows (the dirty trailer, if any), or -1 if the event is malformed.
+template <class Row>
+inline int event_rows(uint32_t const *ev, EventHead const &e, Row &&row)
+{
+    uint32_t const end = e.len;
+    uint32_t const h = ev[0];
+    if ((h & 0xff) == 0xff) {
+        uint32_t const data = h >> 16, bits = (h >> 8) & 31;
+        if (bits > 16) return -1;
+        row(0u, bits, (h >> 13) & 7, &data, bits ? 1u : 0u);
+        return 1;
+    }
+    uint32_t q = 1;
+    for (uint32_t r = 0; r < e.num_rows && r < R433B_BITBUF_ROWS; ++r) {
+        if (q + 1 > end) return -1;
+        uint32_t const w = ev[q];
+        q += 1;
+        if (w >> 31) { // short row
+            uint32_t const data = w & 0xffff, bits = (w >> 16) & 31;
+            if (bits > 16) return -1;
+            row(r, bits, (w >> 21) & 0x3ff, &data, bits ? 1u : 0u);
+            continue;
+        }
+        uint32_t const bits = w & 0xffff;
+        uint32_t words = (bits + 31) / 32;
+        if (e.dirty && r + 1 == e.num_rows) words = ev[end - 1];
+        if (q + words > end) return -1;
+        row(r, bits, w >> 16, ev + q, words);
+        q += words;
+    }
+    return (int)q;
+}
+
 // One event of a pair's byte stream back into the decoder-facing struct
 // (include/bitbuffer.h:34-40).  Row r's bytes go to bb + r*128 and may run on into the
 // following rows exactly as the reference's spill-over does (src/bitbuffer.c:39-54).
@@ -111,38 +157,46 @@ inline int event_to_bitbuffer(uint8_t const *ev8, uint32_t pair_bytes, uint32_t 
     uint32_t const *ev = reinterpret_cast<uint32_t const *>(ev8);
     uint32_t const total = pair_bytes / 4;
     uint32_t pos = 0;
+    EventHead e;
     for (uint32_t i = 0;; ++i) {
         if (pos + 1 > total) return -1;
-        uint32_t h = ev[pos];
-        uint32_t num_rows = h & 0x7f, dirty = (h >> 7) & 1, free_row = (h >> 8) & 0xff, len = h >> 16;
-        if (len < 1 || pos + len > total) return -1;
-        if (i == index) {
-            memset(out, 0, sizeof(*out));
-            out->num_rows = (uint16_t)num_rows;
-            out->free_row = (uint16_t)free_row;
-            uint32_t q = pos + 1;
-            uint32_t const end = pos + len;
-            uint8_t *flat = &out->bb[0][0];
-            for (uint32_t r = 0; r < num_rows && r < R433B_BITBUF_ROWS; ++r) {
-                if (q + 1 > end) return -1;
-                uint32_t bits = ev[q] & 0xffff, syncs = ev[q] >> 16;
-                q += 1;
-                uint32_t words = (bits + 31) / 32;
-                if (dirty && r + 1 == num_rows) words = ev[end - 1];
-                if (q + words > end) return -1;
-                out->bits_per_row[r] = (uint16_t)bits;
-                out->syncs_before_row[r] = (uint16_t)syncs;
-                size_t at = (size_t)r * R433B_BITBUF_COLS;
-                size_t room = sizeof(out->bb) - at;
-                size_t nb = (size_t)words * 4;
-                memcpy(flat + at, ev + q, nb < room ? nb : room);
-                q += words;
-            }
-            if (consumed) *consumed = (pos + len) * 4;
-            return 0;
-        }
-        pos += len;
+        e = event_head(ev[pos]);
+        if (e.len < 1 || pos + e.len > total) return -1;
+        if (i == index) break;
+        pos += e.len;
     }
+    memset(out, 0, sizeof(*out));
+    out->num_rows = (uint16_t)e.num_rows;
+    out->free_row = (uint16_t)e.free_row;
+    uint8_t *flat = &out->bb[0][0];
+    int const rc = event_rows(ev + pos, e, [&](uint32_t r, uint32_t bits, uint32_t syncs, uint32_t const *data, uint32_t words) {
+        out->bits_per_row[r] = (uint16_t)bits;
+        out->syncs_before_row[r] = (uint16_t)syncs;
+        size_t at = (size_t)r * R433B_BITBUF_COLS;
+        size_t room = sizeof(out->bb) - at;
+        size_t nb = (size_t)words * 4;
+        memcpy(flat + at, data, nb < room ? nb : room);
+    });
+    if (rc < 0) return -1;
+    if (consumed) *consumed = (pos + e.len) * 4;
+    return 0;
+}
+
+// The event at ev (head e) appended to `out` in the long form, the only one before one-word rows and events: a
+// header, then every row as a header word and ceil(bits/32) data words, then the dirty trailer.  Returns -1 if the
+// event is malformed.
+inline int event_long_form(uint32_t const *ev, EventHead const &e, std::vector<uint32_t> &out)
+{
+    size_t const at = out.size();
+    out.push_back(0);
+    int const q = event_rows(ev, e, [&](uint32_t, uint32_t bits, uint32_t syncs, uint32_t const *data, uint32_t words) {
+        out.push_back(bits | (syncs << 16));
+        out.insert(out.end(), data, data + words);
+    });
+    if (q < 0) return -1;
+    out.insert(out.end(), ev + q, ev + e.len);
+    out[at] = e.num_rows | (e.dirty << 7) | (e.free_row << 8) | ((uint32_t)(out.size() - at) << 16);
+    return 0;
 }
 
 } // namespace r433b

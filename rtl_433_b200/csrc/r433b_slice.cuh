@@ -16,11 +16,18 @@
 //
 //   event   := u32 { num_rows:7, dirty:1, free_row:8, words:16 }   words = whole event incl. this
 //              row*  [u32 last_row_words  -- only if dirty]
+//            | u32 { 0xff:8, bits:5, syncs:3, data:16 }         one row of <= 16 bits, < 8 syncs
 //   row     := u32 { bits:16, syncs:16 }  then ceil(bits/32) data words (physical row order;
 //              bit i of the row is bit (7 - i%8) of byte i/8, exactly bitbuffer_t's bb layout)
+//            | u32 { data:16, bits:5, syncs:10, 1:1 }         a row of <= 16 bits, < 1024 syncs, not dirty
 //
 // `dirty` marks the reference's 50-row overflow path, which zeroes the last row's length but
 // keeps its bytes (src/bitbuffer.c:118-121): the number of data words then comes from the trailer.
+// The one-word forms carry most events (a noise burst gives one short row): `data` is the row's bytes 0 and 1 as they
+// lie in bb, i.e. the low half of the row's first data word.  Neither can be taken for the long form: a long event's
+// low byte is num_rows <= 50, never 0xff; a long row's top bit is the top bit of syncs, which count at most one sync
+// per symbol of a package, fewer than 2 * kMaxPulses < 2^15.  Only a row of more than 1024 bits spills, and a clean row
+// never gets shorter, so a one-row event of <= 16 bits that is not dirty has free_row 1.
 #pragma once
 #include <stdint.h>
 #include "r433b_core.cuh"
@@ -209,8 +216,14 @@ struct EventWriterT {
         acc = 0;
     }
 
+    // A row of <= 16 bits has flushed no data word yet (row_hw == 0) unless it is the dirty one.
     R4_HD void close_row()
     {
+        if (bits <= 16 && syncs < 1024 && !dirty) {
+            put(row_hdr, (bswap32(acc) & 0xffffu) | (bits << 16) | (syncs << 21) | 0x80000000u);
+            pos = row_hdr + 1;
+            return;
+        }
         if (bits & 31) flush_word();
         put(row_hdr, bits | (syncs << 16));
         pos = row_hdr + 1 + row_hw;
@@ -298,6 +311,7 @@ struct EventWriterT {
     // account_event(): hand the buffer to the decoder, then clear it (src/pulse_slicer.c:26-66)
     R4_HD void emit()
     {
+        bool const one_word = num_rows == 1 && bits <= 16 && syncs < 8 && !dirty;
         if (num_rows == 0) { // an empty buffer is still an event (e.g. nrzs): header only
             ev_start = pos;
             pos += 1;
@@ -306,6 +320,8 @@ struct EventWriterT {
             if (num_rows == 1) gated1++; else gatedN++;
             reset_event();
             return;
+        } else if (one_word) { // nothing of the event is stored yet: its row has no data word before 32 bits
+            pos = ev_start + 1;
         } else {
             close_row();
             if (dirty) { // only the last row can be: its data length travels in a trailer word
@@ -313,7 +329,8 @@ struct EventWriterT {
                 pos += 1;
             }
         }
-        put(ev_start, num_rows | (dirty ? 0x80u : 0u) | (free_row << 8) | ((pos - ev_start) << 16));
+        put(ev_start, one_word ? 0xffu | (bits << 8) | (syncs << 13) | (bswap32(acc) << 16)
+                               : num_rows | (dirty ? 0x80u : 0u) | (free_row << 8) | ((pos - ev_start) << 16));
         committed = pos;
         events++;
         reset_event();
