@@ -91,7 +91,8 @@ struct r433b_ctx {
     cudaStream_t s_in = nullptr, s_det = nullptr, s_out = nullptr;
     static constexpr int kMaxGroups = 16;
     cudaEvent_t ev_in[kMaxGroups]{}, ev_det[kMaxGroups]{}, ev_slc[kMaxGroups]{}, ev_t[4 * kMaxGroups]{}, ev_f[kMaxGroups]{}, ev_init = nullptr;
-    DevBuf d_order; // k_bucket: package indices sorted by (type, length class), per range
+    DevBuf d_order; // k_bucket: package indices sorted by (type, length), per range
+    DevBuf d_sort, d_copy; // k_bucket's tables (SortScratch) and k_slice2's lane-interleaved copy of the widths
     DevBuf d_ranges, d_state, d_lengths, d_stage, d_raw, d_log, d_amoff, d_chunks, d_tiles;
     std::vector<uint64_t> am_offsets; // first sample of stream i in d_am (multiples of the tile), n_streams + 1
     HostBuf h_ranges;
@@ -298,7 +299,7 @@ void r433b_destroy(r433b_ctx *ctx)
     for (DevBuf *b : {&ctx->d_data, &ctx->d_offsets, &ctx->d_train, &ctx->d_pkgs, &ctx->d_ppool, &ctx->d_gpool,
                  &ctx->d_counters, &ctx->d_am, &ctx->d_fm, &ctx->d_devparams, &ctx->d_lists, &ctx->d_pairs,
                  &ctx->d_arena, &ctx->d_cursor, &ctx->d_ranges, &ctx->d_state, &ctx->d_lengths, &ctx->d_stage, &ctx->d_raw, &ctx->d_log, &ctx->d_amoff, &ctx->d_chunks, &ctx->d_tiles,
-                 &ctx->d_order, &ctx->d_an, &ctx->d_an_dev, &ctx->d_an_gap, &ctx->d_an_pairs, &ctx->d_an_arena,
+                 &ctx->d_order, &ctx->d_sort, &ctx->d_copy, &ctx->d_an, &ctx->d_an_dev, &ctx->d_an_gap, &ctx->d_an_pairs, &ctx->d_an_arena,
                  &ctx->d_grab_prior, &ctx->d_grab_segs, &ctx->d_grab_stage})
         if (b->p) cudaFree(b->p);
     for (HostBuf *b : {&ctx->h_pkgs, &ctx->h_ppool, &ctx->h_gpool, &ctx->h_pairs, &ctx->h_events, &ctx->h_ranges})
@@ -414,18 +415,37 @@ int upload_slicer_tables(r433b_ctx *ctx, std::vector<uint32_t> const &rates, cud
     return R433B_OK;
 }
 
+// k_bucket's tables and k_slice2's copy of the widths for ranges of at most `pkgs` packages and `pool_entries` pool
+// entries, reserved next to the pools.  The copy of a range is at most its pool entries plus one group of the
+// longest package per type (r433b_kernels.cuh), so it cannot overflow for the packages the detector stored.  The
+// slice launches of a batch all run on one stream, one range after the other: one copy serves every range.
+int reserve_sort(r433b_ctx *ctx, size_t pkgs, size_t pool_entries, cudaStream_t st)
+{
+    size_t const cap0 = ctx->d_sort.cap;
+    if (int r = dev_reserve(ctx, ctx->d_sort, (4 * kLenBins + pkgs / 32 + 3) * sizeof(unsigned))) return r;
+    // k_bucket_count's histogram starts at zero, and every k_bucket_scan leaves it so
+    if (ctx->d_sort.cap != cap0) CU(cudaMemsetAsync(ctx->d_sort.p, 0, 2 * kLenBins * sizeof(unsigned), st));
+    return dev_reserve(ctx, ctx->d_copy, (pool_entries + 2 * 32 * (size_t)kMaxPulses) * sizeof(PulseGap));
+}
+
 // The slicers over one package range: k_bucket sorts its packages, k_slice2 runs every slicer on them with the
 // tables of sample rate `rate_index`.  `n_pkgs` bounds the range, whose end may only be known on the device.
 void launch_slice(r433b_ctx *ctx, GroupRange *range, unsigned n_pkgs, unsigned rate_index, cudaStream_t st)
 {
+    SortScratch ss;
+    ss.hist = (unsigned *)ctx->d_sort.p;
+    ss.fill = ss.hist + 2 * kLenBins;
+    ss.base = ss.fill + 2 * kLenBins;
+    ss.copy = (PulseGap *)ctx->d_copy.p;
+    ss.copy_cap = std::min<size_t>(ctx->d_copy.cap / sizeof(PulseGap), 0xffffffffu);
     unsigned const n_devs = (unsigned)ctx->devs.size();
     r433b_package *pkgs = (r433b_package *)ctx->d_pkgs.p;
     SliceParams q{};
     q.pkgs = pkgs;
     q.range = range;
     q.order = (unsigned const *)ctx->d_order.p;
-    q.pulse_pool = (int const *)ctx->d_ppool.p;
-    q.gap_pool = (int const *)ctx->d_gpool.p;
+    q.copy = ss.copy;
+    q.group_base = ss.base;
     q.dev = (SlicerParams const *)ctx->d_devparams.p + (size_t)rate_index * n_devs;
     q.n_devs = n_devs;
     q.ook_list = (unsigned const *)ctx->d_lists.p;
@@ -438,16 +458,18 @@ void launch_slice(r433b_ctx *ctx, GroupRange *range, unsigned n_pkgs, unsigned r
     q.cursor = (unsigned long long *)ctx->d_cursor.p;
     q.stage = (uint32_t *)ctx->d_stage.p;
     unsigned const bgrid = (unsigned)ctx->n_sms * 2;
-    R4_LAUNCH(k_bucket_count, bgrid, kBucketThreads, 0, st, range, pkgs, n_pkgs, n_devs);
-    R4_LAUNCH(k_bucket_scan, 1, 1, 0, st, range);
-    R4_LAUNCH(k_bucket_scatter, bgrid, kBucketThreads, 0, st, range, (r433b_package const *)pkgs, n_pkgs, (unsigned *)ctx->d_order.p);
+    R4_LAUNCH(k_bucket_count, bgrid, kBucketThreads, 0, st, range, pkgs, n_pkgs, n_devs, ss.hist);
+    R4_LAUNCH(k_bucket_scan, 1, 32, 0, st, range, ss);
+    R4_LAUNCH(k_bucket_scatter, bgrid, kBucketThreads, 0, st, range, (r433b_package const *)pkgs, n_pkgs, (unsigned *)ctx->d_order.p, ss,
+              (int const *)ctx->d_ppool.p, (int const *)ctx->d_gpool.p);
     R4_LAUNCH(k_slice2, (unsigned)ctx->n_sms * kSliceCtasPerSm, kSliceThreads, 0, st, q);
 }
 
 // The slicer stage over package ranges known on the host: range g (pkg_begin / pkg_end set, the rest zero) uses
-// slicer table g.  Runs again with an event arena grown to what the device counted until every event fits, times
-// the stage with ev[2] -> ev[3] and leaves the event totals in the context.
-int slice_ranges(r433b_ctx *ctx, std::vector<GroupRange> const &ranges, unsigned n_pkgs, cudaStream_t st)
+// slicer table g; the ranges hold `pool_entries` pool entries in all.  Runs again with an event arena grown to what
+// the device counted until every event fits, times the stage with ev[2] -> ev[3] and leaves the event totals in the
+// context.
+int slice_ranges(r433b_ctx *ctx, std::vector<GroupRange> const &ranges, unsigned n_pkgs, size_t pool_entries, cudaStream_t st)
 {
     unsigned const n_devs = (unsigned)ctx->devs.size();
     unsigned long long cursor[4] = {0, 0, 0, 0};
@@ -457,6 +479,7 @@ int slice_ranges(r433b_ctx *ctx, std::vector<GroupRange> const &ranges, unsigned
         size_t const pair_bytes = (size_t)n_pkgs * n_devs * sizeof(r433b_pair);
         if (int r = dev_reserve(ctx, ctx->d_pairs, pair_bytes)) return r;
         if (int r = dev_reserve(ctx, ctx->d_order, (size_t)n_pkgs * sizeof(unsigned))) return r;
+        if (int r = reserve_sort(ctx, n_pkgs, pool_entries, st)) return r;
         if (int r = dev_reserve(ctx, ctx->d_ranges, ranges.size() * sizeof(GroupRange))) return r;
         if (int r = dev_reserve(ctx, ctx->d_cursor, 64)) return r;
         for (int attempt = 0; attempt < 3; ++attempt) {
@@ -759,6 +782,7 @@ int process_iq(r433b_ctx *ctx, r433b_batch const *b, r433b_chain *ch, uint8_t co
         if (int r = dev_reserve(ctx, ctx->d_order, ctx->pkg_cap * sizeof(unsigned))) return r;
         if (int r = dev_reserve(ctx, ctx->d_ppool, ctx->pool_cap * sizeof(int))) return r;
         if (int r = dev_reserve(ctx, ctx->d_gpool, ctx->pool_cap * sizeof(int))) return r;
+        if (int r = reserve_sort(ctx, ctx->pkg_cap, ctx->pool_cap, ctx->s_det)) return r;
         size_t const pair_cap_bytes = ctx->pkg_cap * n_devs * sizeof(r433b_pair);
         if (int r = dev_reserve(ctx, ctx->d_pairs, pair_cap_bytes)) return r;
         if (int r = dev_reserve(ctx, ctx->d_arena, ctx->arena_cap)) return r;
@@ -941,7 +965,7 @@ int process_iq(r433b_ctx *ctx, r433b_batch const *b, r433b_chain *ch, uint8_t co
     ctx->pool_used = counters[1];
     GroupRange all{};
     all.pkg_end = ctx->n_pkgs;
-    if (int r = slice_ranges(ctx, std::vector<GroupRange>{all}, ctx->n_pkgs, st)) return r;
+    if (int r = slice_ranges(ctx, std::vector<GroupRange>{all}, ctx->n_pkgs, ctx->pool_used, st)) return r;
     ctx->n_samples = used_bytes / SS;
     cudaEventElapsedTime(&ctx->timing.h2d_ms, ctx->ev[0], ctx->ev[1]);
     ctx->timing.front_ms = 0;
@@ -1519,7 +1543,7 @@ int r433b_process_pulses(r433b_ctx *ctx, r433b_pulses const *ps)
         size_t const arena_min = ctx->min_caps[2] ? ctx->min_caps[2] : (size_t)(1u << 20);
         if (ctx->arena_cap < arena_min) ctx->arena_cap = arena_min;
         if (int r = upload_slicer_tables(ctx, rates, st)) return r;
-        if (int r = slice_ranges(ctx, ranges, n, st)) return r;
+        if (int r = slice_ranges(ctx, ranges, n, pp.size(), st)) return r;
         ctx->timing.total_ms = ctx->timing.slice_ms;
     }
     ctx->processed = true;

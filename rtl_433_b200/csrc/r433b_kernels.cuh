@@ -2,7 +2,8 @@
 //
 //   k_detect (r433b_detect.cuh) : one WARP per capture stream, IQ -> packages.
 //   k_cf32_to_cs16              : float IQ captures to cs16 in front of k_detect.
-//   k_bucket_count/scan/scatter : the packages of a range sorted by (type, length class) for k_slice2.
+//   k_bucket_count/scan/scatter : the packages of a range sorted by (type, length) for k_slice2, and their widths
+//                                 copied lane-interleaved.
 //   k_slice2                    : one thread per (package, device), a warp = 32 packages of one device: every pulse
 //                                 slicer on every package, events staged per thread and copied into the arena by the warp.
 //   k_mark                      : one-thread bookkeeping between the launches of a pipelined batch.
@@ -45,12 +46,6 @@ __global__ void k_cf32_to_cs16(float4 const *in, uint2 *out, size_t n4)
 
 // ------------------------------------------------------------------------- k_slice2 ------
 
-constexpr int kLenBuckets = 4; // length classes of packages: < 64, < 160, < 400 pulses, longer
-__host__ __device__ inline int len_bucket(unsigned num_pulses)
-{
-    return num_pulses < 64 ? 0 : num_pulses < 160 ? 1 : num_pulses < 400 ? 2 : 3;
-}
-
 // What one pipeline group (a contiguous run of streams) produced, filled on the device so the
 // next stage never waits for the host.
 struct GroupRange {
@@ -58,11 +53,11 @@ struct GroupRange {
     unsigned pool_begin, pool_end;
     unsigned long long arena_begin, arena_end;
     unsigned long long events_end, gated_end;
-    unsigned overflow;
+    unsigned overflow; // bit 0: the detector's arenas, bit 1: the event arena, bit 2: k_slice2's width copy
     unsigned next; // k_slice2 work counter: next (device, package group) item of this range
-    // k_bucket: the packages of the range sorted by (type, length class) in `order[pkg_begin + ...]`
-    unsigned seg_begin[2][kLenBuckets], seg_count[2][kLenBuckets], seg_fill[2][kLenBuckets];
-    unsigned groups[2]; // per type: sum over the buckets of ceil(count / 32)
+    // k_bucket: the packages of the range sorted by type, then by descending num_pulses, in `order[pkg_begin + ...]`:
+    // count[0] OOK packages, then count[1] FSK ones, in groups[t] groups of 32 per type
+    unsigned count[2], groups[2];
 };
 
 __global__ void k_mark(GroupRange *r, int which, unsigned const *counters, unsigned long long const *cursor)
@@ -75,7 +70,6 @@ __global__ void k_mark(GroupRange *r, int which, unsigned const *counters, unsig
         r->pool_end = counters[1];
         r->overflow = counters[2];
         r->next = 0;
-        for (int i = 0; i < 2 * kLenBuckets; ++i) (&r->seg_count[0][0])[i] = 0;
     } else if (which == 2) {
         r->arena_begin = cursor[0];
     } else {
@@ -88,56 +82,153 @@ __global__ void k_mark(GroupRange *r, int which, unsigned const *counters, unsig
 
 // The 32 lanes of a k_slice2 warp are 32 PACKAGES looked at by ONE device.  Lanes that were 32 devices on one
 // package would interpret the same pulse with 32 different sets of limits and so want 32 different things from the
-// bit writer; here all lanes carry the same limits, walk packages of the same type and similar length (k_bucket), and
-// pulse n of one burst is the same kind of thing as pulse n of another -- the lanes differ in data (which bit), far
-// less in control flow.
+// bit writer; here all lanes carry the same limits, walk packages of the same type and length (k_bucket), and pulse
+// n of one burst is the same kind of thing as pulse n of another -- the lanes differ in data (which bit), far less
+// in control flow.  A warp runs until its longest lane is done, so its 32 packages are 32 consecutive ones of the
+// range sorted by length.
+//
+// k_bucket also gives k_slice2 its own copy of the widths, lane-interleaved per group: row k (pulse k and the gap
+// after it) of the package in lane l of group g is copy[base[g] + 32 k + l], so that one step of a warp is one
+// coalesced 256-byte load instead of 64 lines, and the rows of a group are as many as its first (longest) package has
+// entries.  Rows past a shorter package's own entries are padding that no slicer reads.  Groups are sorted by
+// descending length, so group g + 1 has no more rows than any package of the full group g before it: the copy of a
+// type takes at most its pool entries plus 32 x kMaxPulses.
+constexpr unsigned kLenBins = kMaxPulses + 1; // num_pulses 0 .. kMaxPulses
 
-// Sort the packages of a range by (type, length class) into order[pkg_begin ...): count, scan, scatter -- three small
+// num_pulses as a histogram bin (a record that is not a package of this batch -- the stale ones a detector overflow
+// leaves in a range that is redone -- must stay inside the tables), and the rows it takes in the copy: the package's
+// pool entries (r433b_package.pulse_count), where the entry after the last pulse is part of the record
+__host__ __device__ inline unsigned len_bin(unsigned num_pulses) { return num_pulses < kLenBins ? num_pulses : kMaxPulses; }
+__host__ __device__ inline unsigned copy_rows(unsigned len) { return len < (unsigned)kMaxPulses ? len + 1 : kMaxPulses; }
+
+struct SortScratch {
+    unsigned *hist;     // 2 x kLenBins: packages per (type, length); zero between ranges (k_bucket_scan clears it)
+    unsigned *fill;     // 2 x kLenBins: k_bucket_scatter's next position per (type, length)
+    unsigned *base;     // per group, OOK ones first, and one past the last: its first entry in `copy`
+    PulseGap *copy;
+    unsigned long long copy_cap; // entries
+};
+
+// Sort the packages of a range into order[pkg_begin ...) and fill the copy: count, scan, scatter -- three small
 // launches without a block barrier (grid-stride loops; the range is only known on the device).  The count pass also
 // gives every package its row in the pair table.
 constexpr int kBucketThreads = 256;
-__global__ void __launch_bounds__(kBucketThreads) k_bucket_count(GroupRange *r, r433b_package *pkgs, unsigned n_pkgs, unsigned n_devs)
+__global__ void __launch_bounds__(kBucketThreads) k_bucket_count(GroupRange *r, r433b_package *pkgs, unsigned n_pkgs, unsigned n_devs, unsigned *hist)
 {
     unsigned const b0 = r->pkg_begin, b1 = r->pkg_end < n_pkgs ? r->pkg_end : n_pkgs;
     for (unsigned pk = b0 + blockIdx.x * kBucketThreads + threadIdx.x; pk < b1; pk += gridDim.x * kBucketThreads) {
         r433b_package const k = pkgs[pk];
         pkgs[pk].first_pair = pk * n_devs;
-        atomicAdd(&r->seg_count[k.type == 1 ? 0 : 1][len_bucket(k.num_pulses)], 1u);
+        atomicAdd(&hist[(k.type == 1 ? 0 : kLenBins) + len_bin(k.num_pulses)], 1u);
     }
 }
 
-__global__ void k_bucket_scan(GroupRange *r)
+// One warp, on a copy of the histogram in shared memory.  The bins in sorted order (OOK, then FSK; longest first)
+// give every bin its first position; every group of 32 positions takes as many rows as the bin of its first one, and a
+// prefix over the bins of the groups starting in them places the groups in the copy.
+__global__ void __launch_bounds__(32) k_bucket_scan(GroupRange *r, SortScratch s)
 {
-    unsigned at = 0;
-    for (int t = 0; t < 2; ++t) {
-        unsigned g = 0;
-        for (int b = 0; b < kLenBuckets; ++b) {
-            r->seg_begin[t][b] = at;
-            r->seg_fill[t][b] = 0;
-            at += r->seg_count[t][b];
-            g += (r->seg_count[t][b] + 31) / 32;
-        }
-        r->groups[t] = g;
+    constexpr unsigned kBins = 2 * kLenBins, kPer = (kBins + 31) / 32; // consecutive bins of the sorted order per lane
+    __shared__ unsigned hist[kPer * 32];
+    unsigned const lane = threadIdx.x;
+    auto len = [](unsigned i) { return i < kLenBins ? kMaxPulses - i : kLenBins + kMaxPulses - i; }; // i: sorted order
+    for (unsigned i = lane; i < kPer * 32; i += 32) hist[i] = i < kBins ? s.hist[(i < kLenBins ? 0 : kLenBins) + len(i)] : 0;
+    __syncwarp();
+    unsigned n0 = 0, n1 = 0;
+    for (unsigned j = 0; j < kPer; ++j) {
+        unsigned const i = lane * kPer + j;
+        (i < kLenBins ? n0 : n1) += hist[i];
     }
-    r->next = 0;
+    unsigned at = n0 + n1;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        unsigned const v = __shfl_up_sync(0xffffffffu, at, o);
+        if ((int)lane >= o) at += v;
+    }
+    at -= n0 + n1; // first position of the lane's first bin
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        n0 += __shfl_xor_sync(0xffffffffu, n0, o);
+        n1 += __shfl_xor_sync(0xffffffffu, n1, o);
+    }
+    unsigned const g0 = (n0 + 31) / 32, g1 = (n1 + 31) / 32;
+    // the copy entries of the groups whose first position lies in the lane's bins
+    unsigned long long e = 0;
+    for (unsigned j = 0, a = at; j < kPer; ++j) {
+        unsigned const i = lane * kPer + j, n = hist[i];
+        unsigned const q = a - (i < kLenBins ? 0 : n0); // within the type
+        e += (unsigned long long)((q + n + 31) / 32 - (q + 31) / 32) * 32 * copy_rows(len(i));
+        a += n;
+    }
+    unsigned long long incl = e;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        unsigned long long const v = __shfl_up_sync(0xffffffffu, incl, o);
+        if ((int)lane >= o) incl += v;
+    }
+    unsigned long long const total = __shfl_sync(0xffffffffu, incl, 31);
+    // only records that are not this batch's packages (a detector overflow, whose range is redone) can outgrow the
+    // copy: the range then slices nothing
+    bool const fits = total <= s.copy_cap;
+    e = incl - e;
+    for (unsigned j = 0; j < kPer; ++j) {
+        unsigned const i = lane * kPer + j, n = hist[i];
+        if (i >= kBins) break;
+        unsigned const t = i < kLenBins ? 0 : 1, b = t * kLenBins + len(i), q = at - (t ? n0 : 0);
+        s.fill[b] = at;
+        if (n) s.hist[b] = 0;
+        unsigned const size = 32 * copy_rows(len(i));
+        for (unsigned g = (q + 31) / 32; g * 32 < q + n; ++g, e += size) s.base[(t ? g0 : 0) + g] = (unsigned)e;
+        at += n;
+    }
+    if (lane == 0) {
+        s.base[g0 + g1] = (unsigned)total;
+        r->count[0] = n0;
+        r->count[1] = n1;
+        r->groups[0] = fits ? g0 : 0;
+        r->groups[1] = fits ? g1 : 0;
+        if (!fits) r->overflow |= 4;
+        r->next = 0;
+    }
 }
 
-__global__ void __launch_bounds__(kBucketThreads) k_bucket_scatter(GroupRange *r, r433b_package const *pkgs, unsigned n_pkgs, unsigned *order)
+// Every package to its sorted position, and its rows into the copy.  The warp copies its 32 packages one after the
+// other, 32 rows at a time, so that the pool reads are whole lines.
+__global__ void __launch_bounds__(kBucketThreads) k_bucket_scatter(GroupRange *r, r433b_package const *pkgs, unsigned n_pkgs, unsigned *order,
+                                                                  SortScratch s, int const *pulse_pool, int const *gap_pool)
 {
+    unsigned const lane = threadIdx.x & 31;
     unsigned const b0 = r->pkg_begin, b1 = r->pkg_end < n_pkgs ? r->pkg_end : n_pkgs;
-    for (unsigned pk = b0 + blockIdx.x * kBucketThreads + threadIdx.x; pk < b1; pk += gridDim.x * kBucketThreads) {
-        r433b_package const k = pkgs[pk];
-        int const t = k.type == 1 ? 0 : 1, b = len_bucket(k.num_pulses);
-        unsigned const pos = r->seg_begin[t][b] + atomicAdd(&r->seg_fill[t][b], 1u);
-        order[b0 + pos] = pk;
+    unsigned const n0 = r->count[0], g0 = r->groups[0], g1 = r->groups[1];
+    for (unsigned w = b0 + blockIdx.x * kBucketThreads + threadIdx.x - lane; w < b1; w += gridDim.x * kBucketThreads) {
+        unsigned const pk = w + lane;
+        unsigned dst = 0, rows = 0, off = 0;
+        if (pk < b1) {
+            r433b_package const k = pkgs[pk];
+            unsigned const t = k.type == 1 ? 0 : 1, len = len_bin(k.num_pulses);
+            unsigned const pos = atomicAdd(&s.fill[t * kLenBins + len], 1u);
+            order[b0 + pos] = pk;
+            unsigned const q = pos - (t ? n0 : 0);
+            if (q / 32 < (t ? g1 : g0)) {
+                dst = s.base[(t ? g0 : 0) + q / 32] + q % 32;
+                rows = copy_rows(len);
+                off = k.pulse_off;
+            }
+        }
+        for (int l = 0; l < 32; ++l) {
+            unsigned const n = __shfl_sync(0xffffffffu, rows, l), d = __shfl_sync(0xffffffffu, dst, l);
+            unsigned const o = __shfl_sync(0xffffffffu, off, l);
+            for (unsigned k = lane; k < n; k += 32) s.copy[d + 32 * k] = PulseGap{pulse_pool[o + k], gap_pool[o + k]};
+        }
     }
 }
 
 struct SliceParams {
     r433b_package const *pkgs;
-    GroupRange *range; // the packages of the range (k_bucket's segments) and the work counter
+    GroupRange *range; // the packages of the range (k_bucket's counts) and the work counter
     unsigned const *order; // k_bucket's output
-    int const *pulse_pool, *gap_pool;
+    PulseGap const *copy;  // k_bucket's lane-interleaved widths
+    unsigned const *group_base;
     SlicerParams const *dev;  // per device, already scaled to the sample rate of the range
     unsigned n_devs;
     unsigned const *ook_list, *fsk_list; // device indices taking OOK / FSK packages, grouped by modulation
@@ -185,28 +276,15 @@ __global__ void __launch_bounds__(kSliceThreads, kSliceCtasPerSm) k_slice2(Slice
         unsigned const rel = t ? item - items_ook : item;
         unsigned const groups = t ? groups_fsk : groups_ook;
         unsigned const slot = rel / groups;
-        unsigned g = rel - slot * groups;
+        unsigned const g = rel - slot * groups;
         unsigned const dev = (t ? p.fsk_list : p.ook_list)[slot];
-        int b = 0;
-        for (; b < kLenBuckets - 1; ++b) {
-            unsigned const gb = (rg->seg_count[t][b] + 31) / 32;
-            if (g < gb) break;
-            g -= gb;
-        }
-        unsigned const in_seg = g * 32 + lane;
-        bool const active = in_seg < rg->seg_count[t][b];
-        unsigned const pk = active ? p.order[pk_begin + rg->seg_begin[t][b] + in_seg] : 0;
+        unsigned const in_type = g * 32 + lane;
+        bool const active = in_type < rg->count[t];
+        unsigned const pk = active ? p.order[pk_begin + (t ? rg->count[0] : 0) + in_type] : 0;
         SlicerParams const sp = p.dev[dev];
-        PulseView pv;
-        pv.pulse = p.pulse_pool;
-        pv.gap = p.gap_pool;
-        pv.n = 0;
-        if (active) {
-            r433b_package const k = p.pkgs[pk];
-            pv.pulse = p.pulse_pool + k.pulse_off;
-            pv.gap = p.gap_pool + k.pulse_off;
-            pv.n = k.num_pulses;
-        }
+        PulseViewT<32> pv;
+        pv.w = p.copy + p.group_base[(t ? groups_ook : 0) + g] + lane;
+        pv.n = active ? len_bin(p.pkgs[pk].num_pulses) : 0;
         unsigned bytes = 0, nev = 0, ng1 = 0, ngN = 0, wb = 0;
         if (active) {
             EventWriterT<SliceWindow> w;

@@ -340,11 +340,27 @@ using EventWriter = EventWriterT<>;
 
 // ---------------------------------------------------------------------------- slicers ----
 
-struct PulseView {
+// The widths of one package, pulse k and the gap after it as row(k), k < n (row n, where the record has it, is the
+// entry after the last pulse).  Stride 1: the pools, one array of pulses and one of gaps (k_slice_own, the host
+// tests).  Stride S > 1: k_slice2's lane-interleaved copy (r433b_kernels.cuh), where row k of a lane is the pair at
+// w[k * S]: one 8-byte load gives both widths, and the 32 lanes of a warp read one contiguous 256-byte span per step.
+struct alignas(8) PulseGap {
+    int pulse, gap;
+};
+template <unsigned S>
+struct PulseViewT {
+    PulseGap const *w;
+    unsigned n;
+    R4_HD PulseGap row(unsigned k) const { return w[k * S]; }
+};
+template <>
+struct PulseViewT<1> {
     int const *pulse;
     int const *gap;
     unsigned n;
+    R4_HD PulseGap row(unsigned k) const { return PulseGap{pulse[k], gap[k]}; }
 };
+using PulseView = PulseViewT<1>;
 
 enum { // include/r_device.h:24-40
     kModOokMc = 3, kModOokPcm = 4, kModOokPpm = 5, kModOokPwm = 6, kModOokPiwmRaw = 8, kModOokDmc = 9,
@@ -361,7 +377,12 @@ R4_HD bool device_takes(int modulation, int package_type)
 
 R4_HD int iabs(int v) { return v < 0 ? -v : v; }
 R4_HD bool within(int v, int nominal, int tol) { return v >= nominal - tol && v <= nominal + tol; }
-R4_HD int symbol_at(PulseView const &p, unsigned k) { return (k & 1) ? p.gap[k >> 1] : p.pulse[k >> 1]; } // src/pulse_slicer.c:529-535
+template <class PV>
+R4_HD int symbol_at(PV const &p, unsigned k) // src/pulse_slicer.c:529-535
+{
+    PulseGap const r = p.row(k >> 1);
+    return (k & 1) ? r.gap : r.pulse;
+}
 
 // What one iteration of a slicer's main loop does to the bit buffer, in this fixed order.
 enum { kRowNone = 0, kRowAdd, kRowSync, kRowClear, kRowIfOpen };
@@ -391,12 +412,14 @@ struct SlicerState {
 // Move a per-pulse slicer to pulse `k` and issue the loads of its widths now: they are needed one whole step (the
 // front end's classification and the bit writer's work) later, so their latency -- every lane reads another package in
 // k_slice2 -- is off the critical path.
-R4_HD void slicer_advance(PulseView const &p, SlicerState &st, unsigned k)
+template <class PV>
+R4_HD void slicer_advance(PV const &p, SlicerState &st, unsigned k)
 {
     st.k = k;
     if (k < st.total) {
-        st.cv = p.pulse[k];
-        st.cg = p.gap[k];
+        PulseGap const r = p.row(k);
+        st.cv = r.pulse;
+        st.cg = r.gap;
     }
 }
 
@@ -414,8 +437,8 @@ R4_HD int slicer_family(SlicerParams const &t)
     return m == kModFskPwm ? (int)kModOokPwm : m == kModFskPcm ? (int)kModOokPcm : m == kModFskMc ? (int)kModOokMc : m;
 }
 
-template <int MOD>
-R4_HD bool slicer_begin0(PulseView const &p, SlicerParams const &t, SlicerState &st)
+template <int MOD, class PV>
+R4_HD bool slicer_begin0(PV const &p, SlicerParams const &t, SlicerState &st)
 {
     st.k = 0;
     st.cv = st.cg = 0;
@@ -477,11 +500,12 @@ R4_HD bool slicer_begin0(PulseView const &p, SlicerParams const &t, SlicerState 
         if (rz) {
             for (unsigned n = 0; n < N; ++n) { // :105-132
                 int sw = 0, lw = 0, cnt = 0;
-                while (n < N && within(p.pulse[n], t.s_short, tol) && within(p.pulse[n] + p.gap[n], t.s_long, tol)) {
-                    sw += p.pulse[n];
-                    lw += p.pulse[n] + p.gap[n];
+                for (; n < N; ++n) {
+                    PulseGap const r = p.row(n);
+                    if (!within(r.pulse, t.s_short, tol) || !within(r.pulse + r.gap, t.s_long, tol)) break;
+                    sw += r.pulse;
+                    lw += r.pulse + r.gap;
                     cnt++;
-                    n++;
                 }
                 if (cnt >= need) {
                     f_long = fdiv((float)cnt, (float)lw);
@@ -493,9 +517,10 @@ R4_HD bool slicer_begin0(PulseView const &p, SlicerParams const &t, SlicerState 
             if (preamble == 0) { // :134-157
                 int sw = 0, lw = 0, cnt = 0;
                 for (unsigned n = 0; n < N; ++n) {
-                    if (within(p.pulse[n], t.s_short, tol) && within(p.pulse[n] + p.gap[n], t.s_long, tol)) {
-                        sw += p.pulse[n];
-                        lw += p.pulse[n] + p.gap[n];
+                    PulseGap const r = p.row(n);
+                    if (within(r.pulse, t.s_short, tol) && within(r.pulse + r.gap, t.s_long, tol)) {
+                        sw += r.pulse;
+                        lw += r.pulse + r.gap;
                         cnt++;
                     }
                 }
@@ -507,11 +532,13 @@ R4_HD bool slicer_begin0(PulseView const &p, SlicerParams const &t, SlicerState 
         } else {
             for (unsigned n = 0; n < N; ++n) { // :159-180, float product then DOUBLE +0.5
                 int wsum = 0, cnt = 0;
-                while (n < N && (int)dadd((double)fmul((float)p.pulse[n], f_short), 0.5) == 1
-                        && (int)dadd((double)fmul((float)p.gap[n], f_long), 0.5) == 1) {
-                    wsum += p.pulse[n] + p.gap[n];
+                for (; n < N; ++n) {
+                    PulseGap const r = p.row(n);
+                    if ((int)dadd((double)fmul((float)r.pulse, f_short), 0.5) != 1
+                            || (int)dadd((double)fmul((float)r.gap, f_long), 0.5) != 1)
+                        break;
+                    wsum += r.pulse + r.gap;
                     cnt += 2;
-                    n++;
                 }
                 if (cnt >= need) {
                     f_short = f_long = fdiv((float)cnt, (float)wsum);
@@ -522,10 +549,11 @@ R4_HD bool slicer_begin0(PulseView const &p, SlicerParams const &t, SlicerState 
             if (preamble == 0) { // :182-214
                 int wsum = 0, cnt = 0;
                 for (unsigned n = 0; n < N; ++n) {
-                    if (within(p.pulse[n], t.s_short, tol)) { wsum += p.pulse[n]; cnt += 1; }
-                    if (within(p.pulse[n], 2 * t.s_short, tol)) { wsum += p.pulse[n]; cnt += 2; }
-                    if (within(p.gap[n], t.s_long, tol)) { wsum += p.gap[n]; cnt += 1; }
-                    if (within(p.gap[n], 2 * t.s_long, tol)) { wsum += p.gap[n]; cnt += 2; }
+                    PulseGap const r = p.row(n);
+                    if (within(r.pulse, t.s_short, tol)) { wsum += r.pulse; cnt += 1; }
+                    if (within(r.pulse, 2 * t.s_short, tol)) { wsum += r.pulse; cnt += 2; }
+                    if (within(r.gap, t.s_long, tol)) { wsum += r.gap; cnt += 1; }
+                    if (within(r.gap, 2 * t.s_long, tol)) { wsum += r.gap; cnt += 2; }
                 }
                 if (cnt > 20) f_short = f_long = fdiv((float)cnt, (float)wsum);
             }
@@ -556,9 +584,10 @@ R4_HD bool slicer_begin0(PulseView const &p, SlicerParams const &t, SlicerState 
         int pre = 0;
         unsigned n;
         for (n = 0; n < p.n; ++n) {
-            if (p.pulse[n] > half_lo && p.gap[n] > half_lo) {
+            PulseGap const r = p.row(n);
+            if (r.pulse > half_lo && r.gap > half_lo) {
                 pre++;
-                if (p.gap[n] > half_hi) break;
+                if (r.gap > half_hi) break;
             } else {
                 return false;
             }
@@ -567,9 +596,10 @@ R4_HD bool slicer_begin0(PulseView const &p, SlicerParams const &t, SlicerState 
         ++n;
         if (n >= (unsigned)kMaxPulses) return false; // the reference reads past the array here
         // n may equal num_pulses: the entry after the last pulse is part of the package record
-        if (p.pulse[n] < sync_lo || p.gap[n] < sync_lo) return false;
+        PulseGap const sync = p.row(n);
+        if (sync.pulse < sync_lo || sync.gap < sync_lo) return false;
         st.since = 0; // manchester phase
-        if (p.gap[n] > p.pulse[n]) {
+        if (sync.gap > sync.pulse) {
             st.since = 1;
             st.pending = true;
         }
@@ -587,8 +617,8 @@ R4_HD bool slicer_begin0(PulseView const &p, SlicerParams const &t, SlicerState 
     }
 }
 
-template <int MOD>
-R4_HD bool slicer_begin(PulseView const &p, SlicerParams const &t, SlicerState &st)
+template <int MOD, class PV>
+R4_HD bool slicer_begin(PV const &p, SlicerParams const &t, SlicerState &st)
 {
     if (!slicer_begin0<MOD>(p, t, st)) return false;
     slicer_advance(p, st, st.k); // widths of the first pulse the main loop looks at
@@ -596,8 +626,8 @@ R4_HD bool slicer_begin(PulseView const &p, SlicerParams const &t, SlicerState &
 }
 
 // ---- one iteration of the main loop of the slicer -> what it does to the bit buffer
-template <int MOD>
-R4_HD Step slicer_step(PulseView const &p, SlicerParams const &t, SlicerState &st)
+template <int MOD, class PV>
+R4_HD Step slicer_step(PV const &p, SlicerParams const &t, SlicerState &st)
 {
     Step s;
     s.ones = s.zeros = s.post_zeros = 0;
@@ -820,8 +850,8 @@ R4_HD bool slicer_apply(Step const &s, W &w)
     return true;
 }
 
-template <int MOD, class W>
-R4_HD void slice_loop(PulseView const &p, SlicerParams const &t, W &w)
+template <int MOD, class PV, class W>
+R4_HD void slice_loop(PV const &p, SlicerParams const &t, W &w)
 {
     SlicerState st;
     if (!slicer_begin<MOD>(p, t, st)) return;
@@ -831,8 +861,8 @@ R4_HD void slice_loop(PulseView const &p, SlicerParams const &t, W &w)
     }
 }
 
-template <class W>
-R4_HD void slice_dispatch(PulseView const &p, SlicerParams const &t, W &w)
+template <class PV, class W>
+R4_HD void slice_dispatch(PV const &p, SlicerParams const &t, W &w)
 {
     // the four slicers that carry 97 % of the reference's devices get their own loop
     switch (t.modulation) {
