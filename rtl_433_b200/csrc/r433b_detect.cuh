@@ -650,7 +650,8 @@ __device__ R4_NOINLINE void walk_emit(WarpSmem &sm, int type, unsigned long long
     __syncwarp();
 }
 
-__device__ __forceinline__ int am_tile_at(uint16_t const *am16, int n) { return (int)am16[(n >> 6) * (2 * kAmStride) + (n & 63)]; }
+// AM is signed: it dips to about -350 behind a full-scale sample at a block start (x[-1] narrowed to -32768)
+__device__ __forceinline__ int am_tile_at(uint16_t const *am16, int n) { return (int)(int16_t)am16[(n >> 6) * (2 * kAmStride) + (n & 63)]; }
 
 // the IDLE state the noise-floor tracker phases carry in registers
 struct IdleRegs {
@@ -730,7 +731,7 @@ __device__ __forceinline__ int idle_tile(WarpSmem const &sm, IdleRegs &d, int n,
         lo = lo0;
         hi = hi0;
     }
-    uint16_t const *chunk = am16 + lane * (2 * kAmStride);
+    int16_t const *chunk = reinterpret_cast<int16_t const *>(am16) + lane * (2 * kAmStride); // signed, as am_tile_at
     int result = 0;
     bool done = false;
 #pragma unroll 1
@@ -1014,7 +1015,9 @@ __device__ R4_NOINLINE int burst_run(WarpSmem &sm, int n)
             if (L.count && L.start + L.count != rel && L.n == kLogCap) break;
             int cnt = nv_tile - n < 32 ? nv_tile - n : 32;
             int const a = lane < cnt ? am_at(n + lane) : 32767;
-            int const aq = a >> 6; // am >= 0
+            // am >= 0 for the samples taken here: a negative am (behind a full-scale sample at a block start) is below
+            // `down` unless min_level is set far below its default (DESIGN.md section 9)
+            int const aq = a >> 6;
             int const top = __reduce_max_sync(0xffffffffu, lane < cnt ? aq : 0); // one REDUX each
             int hmax = 64 * top + 63;
             hmax = h > hmax ? h : hmax;
@@ -1200,7 +1203,7 @@ __device__ R4_NOINLINE int first_run(WarpSmem &sm, int n)
         cnt = cnt < in_win ? cnt : in_win;
         int const a = lane < cnt ? am_tile_at(am16, n + lane) : 32767;
         int const f = lane < cnt ? (int)(int16_t)sm.fm[fm_pidx((int)(pos - sm.win0) + lane)] : 0;
-        int const aq = a >> 6;
+        int const aq = a >> 6; // am >= 0 here, as in burst_run
         int const top = __reduce_max_sync(0xffffffffu, lane < cnt ? aq : 0);
         int hmax = 64 * top + 63;
         hmax = d.high > hmax ? d.high : hmax;

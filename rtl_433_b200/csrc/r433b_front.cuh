@@ -386,7 +386,9 @@ __global__ void __launch_bounds__(kFrontWarps * 32, kFrontCtasPerSm) k_front(Fro
                     yy = yb;
                     cmin = min(cmin, min(ya, yb));
                     cmax = max(cmax, max(ya, yb));
-                    o[j >> 1] = (uint32_t)ya | ((uint32_t)yb << 16);
+                    // AM dips below zero behind a full-scale sample at a block start (x[-1] narrowed to -32768):
+                    // ya is cut to 16 bits so that its sign does not spill over yb
+                    o[j >> 1] = (uint32_t)(uint16_t)ya | ((uint32_t)yb << 16);
                 }
                 if (SS == 2) {
                     uint4 v;

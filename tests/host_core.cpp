@@ -375,13 +375,15 @@ int hc_check_pulse_bound(unsigned seed, int trials)
         Levels lv = compute_levels(0, (t % 5 == 0) ? -10.0f : 0.0f, -12.1442f - (float)(t % 7), 9.0f);
         int const minh = lv.min_high;
         int h = minh + rand() % 30000;
-        int low = rand() % 4000;
-        int base = rand() % 32000, spread = 1 + rand() % (t % 3 ? 400 : 20000);
+        // AM reaches below zero (to about -350) behind a full-scale sample at a block start, and `low` follows it
+        // down; [-2400, 32767] covers the filter's whole reachable range with a margin
+        int low = -2401 + rand() % 6400;
+        int base = -2400 + rand() % 34400, spread = 1 + rand() % (t % 3 ? 400 : 20000);
         int a[32], top = -512;
         for (int j = 0; j < 32; ++j) {
             int v = base + rand() % spread - spread / 2;
-            a[j] = v < 0 ? 0 : (v > 32767 ? 32767 : v);
-            if (a[j] / 64 > top) top = a[j] / 64;
+            a[j] = v < -2400 ? -2400 : (v > 32767 ? 32767 : v);
+            if ((a[j] >> 6) > top) top = a[j] >> 6; // as k_detect bounds it
         }
         int hmax = 64 * top + 63;
         if (h > hmax) hmax = h;

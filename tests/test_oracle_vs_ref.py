@@ -42,6 +42,22 @@ def test_ook_stream_all_devices(ref, seed):
     assert not helpers.compare_results(want, hc.run(x, 2), "device functions", floats=False)
 
 
+@pytest.mark.parametrize("seed", range(4))
+def test_full_scale_samples_at_block_starts(ref, seed):
+    """The hostile-IQ fuzz's (255, 255) family (tests/hostile_iq.py): the reference's int16 x[-1] across block calls
+    drives AM below zero behind a spike on the last sample of a block.  The oracle must follow it exactly."""
+    import hostile_iq
+    devs = ref.registered()
+    x = hostile_iq.spikes(seed)[0].iq
+    o = orc.Oracle(store_bitbuffers=False, store_stages=True)
+    o.add_devices(devs)
+    for bb, block in ((0, hostile_iq.DEFAULT_BLOCK), (32768, hostile_iq.SMALL_BLOCK)):
+        want = ref.run(x, 2, block_bytes=bb)
+        assert hostile_iq.block_start_dips(want["am"], block).min() < 0
+        d = helpers.compare_results(want, o.run(x, 2, block_bytes=bb), f"oracle, block_bytes {bb}")
+        assert not d, "\n".join(d[:12])
+
+
 @pytest.mark.parametrize("fpdm,freq", [(2, 868000000), (0, 433920000)])
 def test_fsk_stream_all_devices(ref, fpdm, freq):
     devs = ref.registered()
