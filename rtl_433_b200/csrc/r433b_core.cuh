@@ -156,7 +156,16 @@ struct Levels {
     int min_high;   // :33
     int ratio;      // :34
     int max_high;   // :24 OOK_MAX_HIGH_LEVEL
+    int monotone;   // derived_high() is non-decreasing in `low` over its whole range (compute_levels proves it)
 };
+
+// `high` as IDLE derives it from `low` (src/pulse_detect.c:331-332).  ratio * low is int multiplication in the
+// reference: above min_snr ~48 dB (envelope) it wraps in 32 bits, as it does on the hardware the reference runs on.
+R4_HD int derived_high(int low, Levels const &lv)
+{
+    int const h = (int)((unsigned)lv.ratio * (unsigned)low);
+    return h < lv.min_high ? lv.min_high : h;
+}
 
 enum { kIdle = 0, kPulse = 1, kGapStart = 2, kGap = 3 };
 enum { kFskInit = 0, kFskHigh = 1, kFskLow = 2, kFskErr = 3 };
@@ -245,6 +254,19 @@ R4_HD void fsk_shift(D &d, Trains const &t, Ctx &cx)
     d.fsk_hw = kMaxPulses;
 }
 
+// A train entry read back by a warp-uniform step.  Every lane writes the same entries, and nothing but a collective
+// keeps the lanes of a warp at the same sample: without the first sync a lane could read an entry before a slower lane
+// has written it for this sample, without the second a faster lane could overwrite it for a later sample before a
+// slower one has read it (first_run feeds the FSK sub-detector up to 32 samples per trip with no collective between).
+template <class Ctx>
+R4_HD int train_read(int const *arr, unsigned i, Ctx &cx)
+{
+    cx.sync();
+    int const v = arr[i];
+    cx.sync();
+    return v;
+}
+
 // src/pulse_detect_fsk.c:34-141
 template <class D, class Ctx>
 R4_HD void fsk_classic(D &d, Trains const &t, int v, Ctx &cx)
@@ -281,9 +303,9 @@ R4_HD void fsk_classic(D &d, Trains const &t, int v, Ctx &cx)
                 put(t.fsk_pulse, d.fsk_hw, d.fsk_n, (int)d.fk_len);
                 d.fk_len = 0;
             } else {
-                d.fk_len += (unsigned)t.fsk_gap[d.fsk_n - 1];
+                d.fk_len += (unsigned)train_read(t.fsk_gap, d.fsk_n - 1, cx);
                 d.fsk_n -= 1;
-                if (d.fsk_n == 0 && t.fsk_pulse[0] == 0) {
+                if (d.fsk_n == 0 && train_read(t.fsk_pulse, 0, cx) == 0) {
                     d.fk_f1 = d.fk_f2;
                     d.fk_st = kFskInit;
                 }
@@ -301,7 +323,7 @@ R4_HD void fsk_classic(D &d, Trains const &t, int v, Ctx &cx)
                 d.fk_len = 0;
                 if (d.fsk_n >= (unsigned)kMaxPulses) fsk_shift(d, t, cx);
             } else {
-                d.fk_len += (unsigned)t.fsk_pulse[d.fsk_n];
+                d.fk_len += (unsigned)train_read(t.fsk_pulse, d.fsk_n, cx);
                 if (d.fsk_n == 0) d.fk_st = kFskInit;
             }
         } else {
@@ -376,14 +398,21 @@ R4_HD Thresholds det_thresholds(int low, int high, Levels const &lv)
     return r;
 }
 
+// The lowest trigger level IDLE can reach while `low` stays >= lmin and `high` is derived from it (k_detect's IDLE
+// shortcuts): `up` grows with `low` and with `high`, so it is the one at lmin where derived_high() is monotone
+// (Levels::monotone), otherwise the one with `high` at its floor min_high
+R4_HD int lowest_up(int lmin, Levels const &lv)
+{
+    return det_thresholds(lmin, lv.monotone ? derived_high(lmin, lv) : lv.min_high, lv).up;
+}
+
 // one IDLE sample that does not start a package (src/pulse_detect.c:325-334)
 R4_HD void idle_track(DetState &d, Levels const &lv, int a)
 {
     int delta = a - d.low;
     d.low += delta / 1024;
     d.low += delta > 0 ? 1 : -1;
-    d.high = lv.ratio * d.low;
-    if (d.high < lv.min_high) d.high = lv.min_high;
+    d.high = derived_high(d.low, lv);
     if (d.lead_in <= kLeadIn) d.lead_in += 1;
 }
 
@@ -431,7 +460,7 @@ R4_HD void close_fsk(DetState &d, Trains const &t, int fpdm)
 // package ends, from the logged samples: r433b_detect.cuh).  `f` is then only looked at while
 // ook_n == 0 (the FSK sub-detector and the estimate of the first pulse).
 //
-// Mode kStepLean compiles the FSK sub-detector out: valid whenever ook_n != 0 or the state is IDLE / GAP.
+// Mode kStepLean compiles the FSK sub-detector out: valid whenever fsk_n <= 16 and ook_n != 0 or the state is IDLE / GAP.
 // Mode kStepFirst only has the PULSE / GAP_START branches: valid inside a first pulse (ook_n == 0).  k_detect
 // keeps the lean instance on its hot path and enters the other only inside first pulses; kStepAll is everything.
 enum { kStepF1Deferred = 4 };
@@ -486,7 +515,9 @@ R4_HD int det_step(DetState &d, Levels const &lv, Trains const &t, int a, int f,
                 d.st = kPulse;
             } else if (d.run >= kMinPulseSamples) {
                 d.st = kGap;
-                if (WithFsk && d.fsk_n > (unsigned)kMinPulses) { // only the first pulse feeds the FSK train: later gaps find fsk_n <= 16 (else the package ended here)
+                // only the first pulse and its GAP_START feed the FSK train, but that GAP_START feeds it once more on the
+                // sample it moves to GAP: a later GAP_START can find fsk_n > 16 too (k_detect then keeps out of burst_run)
+                if (WithFsk && d.fsk_n > (unsigned)kMinPulses) {
                     close_fsk(d, t, fpdm);
                     return 2;
                 }

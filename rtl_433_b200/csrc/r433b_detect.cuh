@@ -658,13 +658,6 @@ struct IdleRegs {
     int low, high, lead_in;
 };
 
-// `high` as IDLE derives it from `low` (src/pulse_detect.c:331-332)
-__device__ __forceinline__ int derived_high(int low, Levels const &lv)
-{
-    int const h = lv.ratio * low;
-    return h < lv.min_high ? lv.min_high : h;
-}
-
 // IDLE over a long stretch of the tile in sm.am from sample n on, lane-parallel: see the comment in the file header
 // and below.  While |am - low| < 1024 the tracker is low += (am > low) ? +1 : -1, so low keeps the parity of
 // (low0 + samples seen) and two trajectories of equal parity never cross and merge once the data passes between
@@ -699,9 +692,9 @@ __device__ __forceinline__ int idle_tile(WarpSmem const &sm, IdleRegs &d, int n,
     }
     int Lmin = lo0 < pmin - 1 ? lo0 : pmin - 1;
     int Lmax = hi0 > pmax ? hi0 : pmax;
-    Thresholds th = det_thresholds(Lmin, derived_high(Lmin, lv), lv);
+    int const up = lowest_up(Lmin, lv);
     bool const armed = d.lead_in + (nv_tile - n) > kLeadIn;
-    bool ok = in_region && !(armed && cmax > th.up) && (pmax - Lmin < 1024) && (Lmax - pmin < 1024);
+    bool ok = in_region && !(armed && cmax > up) && (pmax - Lmin < 1024) && (Lmax - pmin < 1024);
     unsigned bad = ~__ballot_sync(0xffffffffu, ok) & (0xffffffffu << c0);
     int const e = bad ? __ffs(bad) - 1 : 32; // chunks c0 .. e-1 form the stretch
     if (e - c0 < 2) return 0;
@@ -794,9 +787,9 @@ __device__ R4_NOINLINE int idle_run(WarpSmem &sm, int n)
         int cnt = nv_tile - n < 32 ? nv_tile - n : 32;
         int a = lane < cnt ? am_at(n + lane) : -32768;
         int lmin = d.low - cnt;
-        Thresholds th = det_thresholds(lmin, derived_high(lmin, lv), lv); // lowest trigger level reachable in this chunk
+        int const up = lowest_up(lmin, lv); // lowest trigger level reachable in this chunk
         bool armed = d.lead_in + cnt - 1 > kLeadIn;
-        bool stop = lane < cnt && ((armed && a > th.up) || (a - lmin >= 1024) || (d.low + cnt - a >= 1024));
+        bool stop = lane < cnt && ((armed && a > up) || (a - lmin >= 1024) || (d.low + cnt - a >= 1024));
         unsigned m = __ballot_sync(0xffffffffu, stop);
         if (m) {
             int first = __ffs(m) - 1;
@@ -906,7 +899,7 @@ __device__ R4_NOINLINE unsigned long long idle_skip(WarpSmem &sm, int16_t const 
         int const Lmax = bhi > tmax ? bhi : tmax;
         bool const armed = li + T > kLeadIn;
         bool const ok = inside && iir16_nowrap(yin, a1, b0, ti.xsum) == (int)ti.first && tmax - Lmin < 1024
-                && Lmax - tmin < 1024 && !(armed && tmax > det_thresholds(Lmin, derived_high(Lmin, lv), lv).up);
+                && Lmax - tmin < 1024 && !(armed && tmax > lowest_up(Lmin, lv));
         unsigned const bad = ~__ballot_sync(0xffffffffu, ok);
         int const e = bad ? __ffs(bad) - 1 : 32; // tiles t .. t + e - 1 are skipped
         if (e == 0) break;
@@ -1015,13 +1008,14 @@ __device__ R4_NOINLINE int burst_run(WarpSmem &sm, int n)
             if (L.count && L.start + L.count != rel && L.n == kLogCap) break;
             int cnt = nv_tile - n < 32 ? nv_tile - n : 32;
             int const a = lane < cnt ? am_at(n + lane) : 32767;
-            // am >= 0 for the samples taken here: a negative am (behind a full-scale sample at a block start) is below
-            // `down` unless min_level is set far below its default (DESIGN.md section 9)
-            int const aq = a >> 6;
+            // am / 64 as :362 computes it: AM dips below zero behind a full-scale sample at a block start, and such a
+            // sample is taken here when `down` is negative (`low` below zero, min_level far below its default)
+            int const aq = a / 64;
             int const top = __reduce_max_sync(0xffffffffu, lane < cnt ? aq : 0); // one REDUX each
             int hmax = 64 * top + 63;
             hmax = h > hmax ? h : hmax;
-            unsigned const m = __ballot_sync(0xffffffffu, lane < cnt && a < det_thresholds(low, hmax, lv).down);
+            int const dn = det_thresholds(low, hmax, lv).down;
+            unsigned const m = __ballot_sync(0xffffffffu, lane < cnt && a < dn);
             if (m) cnt = __ffs(m) - 1;
             if (cnt) {
                 __syncwarp();
@@ -1029,14 +1023,14 @@ __device__ R4_NOINLINE int burst_run(WarpSmem &sm, int n)
                 __syncwarp();
                 // h >= min_high >= 0 here, so h / 64 == h >> 6.  Eight steps per trip, the loops kept rolled: seven
                 // warps per scheduler share an instruction cache of a few hundred instructions.
-                // q >= 0, so one step takes at most h >> 6 off, and less from a lower h: after k steps h is still
-                // >= h0 - k (h0 >> 6).  If that stays >= min_high over the whole stretch the clamp of :363 cannot act
-                // and is left out of the dependency chain.
+                // With dn >= 0 every sample taken has q >= 0, so one step takes at most h >> 6 off, and less from a
+                // lower h: after k steps h is still >= h0 - k (h0 >> 6).  If that stays >= min_high over the whole
+                // stretch the clamp of :363 cannot act and is left out of the dependency chain.
                 int4 const *qp = reinterpret_cast<int4 const *>(sm.q);
                 int trips = cnt >> 3;
 #define R4_STEP(q) h += (q) - (int)((unsigned)h >> 6)
 #define R4_STEP_CLAMPED(q) h = max(h + (q) - (int)((unsigned)h >> 6), minh)
-                if (h - cnt * (int)((unsigned)h >> 6) >= minh) {
+                if (dn >= 0 && h - cnt * (int)((unsigned)h >> 6) >= minh) {
 #pragma unroll 1
                     for (; trips > 0; --trips, qp += 2) {
                         int4 const b = qp[0], c = qp[1];
@@ -1073,7 +1067,7 @@ __device__ R4_NOINLINE int burst_run(WarpSmem &sm, int n)
                     run = 0;
                     st = kGapStart;
                 } else {
-                    h += (aj >> 6) - (int)((unsigned)h >> 6);
+                    h += aj / 64 - (int)((unsigned)h >> 6);
                     h = h < minh ? minh : h;
                     log_add(L, log, (unsigned)(t0 + (unsigned long long)n - d.start_abs), 1u, lane);
                     run += 1;
@@ -1203,7 +1197,7 @@ __device__ R4_NOINLINE int first_run(WarpSmem &sm, int n)
         cnt = cnt < in_win ? cnt : in_win;
         int const a = lane < cnt ? am_tile_at(am16, n + lane) : 32767;
         int const f = lane < cnt ? (int)(int16_t)sm.fm[fm_pidx((int)(pos - sm.win0) + lane)] : 0;
-        int const aq = a >> 6; // am >= 0 here, as in burst_run
+        int const aq = a / 64; // as in burst_run
         int const top = __reduce_max_sync(0xffffffffu, lane < cnt ? aq : 0);
         int hmax = 64 * top + 63;
         hmax = d.high > hmax ? d.high : hmax;
@@ -1532,7 +1526,9 @@ __global__ void __launch_bounds__(kDetectWarps * 32, kDetectCtasPerSm) k_detect(
             int m = n;
             if (st == kIdle)
                 m = idle_run(sm, n);
-            else if (defer_f1 && !sm.ws.d.eop_flag && (sm.ws.d.ook_n != 0 || st == kGap))
+            // burst_run leaves out the FSK hand-over of GAP_START (:387): the first pulse's GAP_START may feed the FSK
+            // sub-detector its 17th pulse on the sample it moves to GAP, and then the next GAP_START ends the package
+            else if (defer_f1 && !sm.ws.d.eop_flag && (sm.ws.d.ook_n != 0 || st == kGap) && sm.ws.d.fsk_n <= (unsigned)kMinPulses)
                 m = burst_run(sm, n);
             else if (st == kPulse && sm.ws.d.ook_n == 0)
                 m = first_run<SS>(sm, n);

@@ -15,7 +15,23 @@
 
 namespace r433b {
 
-// include/baseband.h:43-46 with _exp10f(x) = powf(10, x); src/pulse_detect.c:86-98, :24
+// Whether k_detect's IDLE shortcuts (idle_tile, idle_fast, idle_skip) may bound the lowest trigger level over a
+// range [Lmin, Lmax] of `low` by the one at Lmin.  The trigger level up(low, derived_high(low)) of det_thresholds()
+// is non-decreasing in `low` whenever derived_high() is, so this proves
+//     derived_high(l, lv) <= derived_high(l + 1, lv)   for every l in [kLowMin, kLowMax)
+// by exhaustion.  `low` tracks int16 AM one step at a time and never leaves [-32769, 32768].  It fails only where
+// ratio * low wraps in 32 bits: ratio > 65536, i.e. min_snr above ~48.2 dB (envelope) or ~96.3 dB (magnitude).
+// Without it the shortcuts bound derived_high() from below by min_high, which holds for every Levels.
+inline int levels_monotone(Levels const &lv)
+{
+    constexpr int kLowMin = -32769, kLowMax = 32768;
+    for (int l = kLowMin; l < kLowMax; ++l)
+        if (derived_high(l, lv) > derived_high(l + 1, lv)) return 0;
+    return 1;
+}
+
+// include/baseband.h:43-46 with _exp10f(x) = powf(10, x); src/pulse_detect.c:86-98, :24.  At min_snr = 99 dB in
+// envelope mode the ratio (7.9e9) does not fit an int: the conversion gives INT_MIN on x86, as in the reference.
 inline Levels compute_levels(int use_mag, float level_limit, float min_level, float min_snr)
 {
     Levels lv;
@@ -29,6 +45,7 @@ inline Levels compute_levels(int use_mag, float level_limit, float min_level, fl
         lv.ratio = (int)(0.5 + powf(10, min_snr / 10.0f));
     }
     lv.max_high = (int)(powf(10, (0 + 42.1442f) / 10.0f));
+    lv.monotone = levels_monotone(lv);
     return lv;
 }
 

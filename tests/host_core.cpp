@@ -372,7 +372,10 @@ int hc_check_pulse_bound(unsigned seed, int trials)
     srand(seed);
     int bad = 0;
     for (int t = 0; t < trials; ++t) {
-        Levels lv = compute_levels(0, (t % 5 == 0) ? -10.0f : 0.0f, -12.1442f - (float)(t % 7), 9.0f);
+        // min_level down to -99 dB (min_high 0), min_snr up to 99 dB (ratio * low wraps)
+        static float const min_levels[] = {-12.1442f, -13.1442f, -18.1442f, -35.0f, -42.0f, -60.0f, -99.0f};
+        static float const min_snrs[] = {9.0f, 1.0f, 60.0f, 99.0f};
+        Levels lv = compute_levels(t % 11 == 0, (t % 5 == 0) ? -10.0f : 0.0f, min_levels[t % 7], min_snrs[t / 7 % 4]);
         int const minh = lv.min_high;
         int h = minh + rand() % 30000;
         // AM reaches below zero (to about -350) behind a full-scale sample at a block start, and `low` follows it
@@ -383,7 +386,7 @@ int hc_check_pulse_bound(unsigned seed, int trials)
         for (int j = 0; j < 32; ++j) {
             int v = base + rand() % spread - spread / 2;
             a[j] = v < -2400 ? -2400 : (v > 32767 ? 32767 : v);
-            if ((a[j] >> 6) > top) top = a[j] >> 6; // as k_detect bounds it
+            if (a[j] / 64 > top) top = a[j] / 64; // as k_detect bounds it
         }
         int hmax = 64 * top + 63;
         if (h > hmax) hmax = h;
@@ -396,6 +399,29 @@ int hc_check_pulse_bound(unsigned seed, int trials)
         }
         if (h > hmax) bad++;
     }
+    return bad;
+}
+
+// k_detect's IDLE shortcuts: lowest_up(lmin) is no higher than the trigger level of any `low` >= lmin with `high`
+// derived from it, for every Levels -- including those where ratio * low wraps (Levels::monotone == 0).  Levels
+// (mode, level_limit, min_level, min_snr) come in `grid` as 4 floats each.  Returns the number of violations, or -1
+// when `want_nonmonotone` of the grid points do not have monotone == 0 (the check must reach that branch).
+int hc_check_idle_bound(unsigned seed, float const *grid, int n_levels, int trials, int want_nonmonotone)
+{
+    srand(seed);
+    int bad = 0, nonmono = 0;
+    for (int g = 0; g < n_levels; ++g) {
+        Levels lv = compute_levels((int)grid[4 * g], grid[4 * g + 1], grid[4 * g + 2], grid[4 * g + 3]);
+        nonmono += !lv.monotone;
+        // exhaustive in `low` near the wrap points and the sign change, random elsewhere
+        for (int t = 0; t < trials; ++t) {
+            int lmin = t < 4096 ? -2048 + t : -32769 + rand() % 65537;
+            int l = lmin + (t & 1 ? rand() % 64 : rand() % 4096);
+            if (l > 32768) l = 32768;
+            if (lowest_up(lmin, lv) > det_thresholds(l, derived_high(l, lv), lv).up) bad++;
+        }
+    }
+    if (nonmono < want_nonmonotone) return -1;
     return bad;
 }
 

@@ -5,6 +5,11 @@ size and at block_bytes = 32768, and must equal the oracle exactly: packages, wi
 arrays (and the compiled reference when it is present).  Each family also asserts that it reached the path it aims
 at, so that a family which stops reaching it fails.  tests/test_emu_front_fuzz.py runs the same bodies under the SIMT
 emulator with fewer seeds."""
+import concurrent.futures
+import functools
+import os
+import threading
+
 import numpy as np
 import pytest
 
@@ -51,15 +56,38 @@ def _groups(cases):
     return out.values()
 
 
-def run_family(ctx, devices, name, seeds, blocks=BLOCKS, levels=None, evidence=True):
+@functools.lru_cache(maxsize=None)
+def family_cases(name, seed):
+    """The cases of one family and seed, made once per process (the level fuzz runs them at many levels)."""
+    return tuple(H.FAMILIES[name][0](seed))
+
+
+def oracle_results(devices, cases, blocks, levels=None):
+    """The oracle's result of every case at every block size, {(id(case), block_bytes): result}, on a few host threads
+    (the oracle holds no global state and its calls release the interpreter lock)."""
+    local = threading.local()
+
+    def one(job):
+        c, bb = job
+        if not hasattr(local, "o"):
+            local.o = oracle_for(devices)
+            if levels:
+                local.o.set_levels(**levels)
+        return (id(c), bb), local.o.run(c.iq, c.fmt, c.rate, c.freq, c.fpdm, block_bytes=bb)
+
+    with concurrent.futures.ThreadPoolExecutor(min(8, os.cpu_count() or 1)) as ex:
+        return dict(ex.map(one, [(c, bb) for c in cases for bb in blocks]))
+
+
+def run_family(ctx, devices, name, seeds, blocks=BLOCKS, levels=None, evidence=True, collect=None):
     """Every case of family `name` over `seeds` through run_gpu against the oracle; the evidence checks run on the
-    default levels only (magnitude mode, for one, never reaches envelope 32768)."""
-    gen, ev = H.FAMILIES[name]
-    cases = [c for s in seeds for c in gen(s)]
-    o = oracle_for(devices)
+    default levels only (magnitude mode, for one, never reaches envelope 32768).  `collect`, a list, receives
+    (case, block_bytes, oracle result) of every comparison."""
+    ev = H.FAMILIES[name][1]
+    cases = [c for s in seeds for c in family_cases(name, s)]
+    wants = oracle_results(devices, cases, blocks, levels)
     if levels:
         ctx.set_levels(**levels)
-        o.set_levels(**levels)
     try:
         for group in _groups(cases):
             c0 = group[0]
@@ -67,8 +95,10 @@ def run_family(ctx, devices, name, seeds, blocks=BLOCKS, levels=None, evidence=T
                 gpu = run_gpu(ctx, [c.iq for c in group], c0.fmt, c0.rate, c0.freq, c0.fpdm, bb)
                 tm = ctx.timing()
                 for c, g in zip(group, gpu):
-                    want = o.run(c.iq, c.fmt, c.rate, c.freq, c.fpdm, block_bytes=bb)
+                    want = wants[(id(c), bb)]
                     check(g, want, f"{c} block_bytes {bb} levels {levels}")
+                    if collect is not None:
+                        collect.append((c, bb, want))
                     if evidence and not levels:
                         blk = (bb or 262144) // c.fmt
                         if name in H.TIMED:
@@ -81,17 +111,25 @@ def run_family(ctx, devices, name, seeds, blocks=BLOCKS, levels=None, evidence=T
     return cases
 
 
-def against_reference(ctx, cases):
-    """The same batches against the compiled reference, where it is present."""
+def against_reference(ctx, cases, levels=None):
+    """The same batches against the compiled reference, where it is present (at the default levels or `levels`)."""
     if not refh.available():
         return
     r = refh.Ref(store_bitbuffers=False, store_stages=True)
     r.register_defaults()
-    for group in _groups(cases):
-        c0 = group[0]
-        gpu = run_gpu(ctx, [c.iq for c in group], c0.fmt, c0.rate, c0.freq, c0.fpdm)
-        for c, g in zip(group, gpu):
-            check(g, r.run(c.iq, c.fmt, c.rate, c.freq, c.fpdm), f"{c} vs reference")
+    if levels:
+        ctx.set_levels(**levels)
+        r.set_levels(**levels)
+    try:
+        for group in _groups(cases):
+            c0 = group[0]
+            gpu = run_gpu(ctx, [c.iq for c in group], c0.fmt, c0.rate, c0.freq, c0.fpdm)
+            for c, g in zip(group, gpu):
+                check(g, r.run(c.iq, c.fmt, c.rate, c.freq, c.fpdm), f"{c} vs reference levels {levels}")
+    finally:
+        r.close()
+        if levels:
+            ctx.set_levels()
 
 
 def family(ctx, devices, name, seeds):
@@ -107,11 +145,22 @@ def levels(ctx, devices, seeds):
         run_family(ctx, devices, name, seeds, blocks=(0, 32768), levels=dict(level_limit=-8.0))
 
 
-def pipelined_and_chained(ctx, devices, seeds):
+def pipelined_and_chained(ctx, devices, seeds, levels=None):
     """Full-scale spikes and glitches through the pipelined host path (time slices, state carried between launches)
-    and as chained batches cut at block boundaries (state carried between calls)."""
-    cases = [c for s in seeds for n in ("spikes", "glitches") for c in H.FAMILIES[n][0](s)]
+    and as chained batches cut at block boundaries (state carried between calls), at the default levels or `levels`."""
+    cases = [c for s in seeds for n in ("spikes", "glitches") for c in family_cases(n, s)]
     o = oracle_for(devices, stages=True)
+    if levels:
+        ctx.set_levels(**levels)
+        o.set_levels(**levels)
+    try:
+        _pipelined_and_chained(ctx, cases, o)
+    finally:
+        if levels:
+            ctx.set_levels()
+
+
+def _pipelined_and_chained(ctx, cases, o):
     for bb in BLOCKS:
         wants = [o.run(c.iq, 2, block_bytes=bb) for c in cases]
         data = np.concatenate([c.iq for c in cases])

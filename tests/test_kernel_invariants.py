@@ -21,6 +21,19 @@ def test_pulse_threshold_bound():
     assert _lib().hc_check_pulse_bound(1, 200000) == 0
 
 
+def test_idle_trigger_bound_on_the_level_grid():
+    """IDLE shortcuts: lowest_up(lmin) never lies above the trigger level of a `low` >= lmin, at every level of the
+    level fuzz's grid -- among them the min_snr settings where ratio * low wraps and derived_high() is not monotone."""
+    import test_level_fuzz as lf
+    grid = [dict(lf.DEFAULT, **g) for g in lf.GRID]
+    flat = np.array([[g["use_mag_est"], g["level_limit"], g["min_level"], g["min_snr"]] for g in grid], np.float32)
+    L = _lib()
+    L.hc_check_idle_bound.argtypes = [C.c_uint, C.c_void_p, C.c_int, C.c_int, C.c_int]
+    # not monotone: envelope mode at 50 and 60 dB, magnitude mode at 99 dB (envelope mode at 99 dB has ratio INT_MIN,
+    # which makes every ratio * low 0 or INT_MIN: `high` is min_high throughout)
+    assert L.hc_check_idle_bound(3, flat.ctypes.data, len(grid), 20000, 3) == 0
+
+
 def test_fm_filter_state_rebuild_is_sound_and_usually_converges():
     """FM on demand: monotone filter => once the two extreme start states meet, all states have met.
     A live (noisy) discriminator makes them meet within one 1024/512-sample tile; an exactly

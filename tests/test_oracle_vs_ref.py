@@ -169,3 +169,31 @@ def test_per_stage_functions(ref):
         L.refh_demod_fm(cs16, src.ctypes.data, a.ctypes.data, 5000, 1024000 if cs16 else 250000, lp, ca.ctypes.data)
         O.orc_demod_fm(cs16, src.ctypes.data, b.ctypes.data, 5000, 1024000 if cs16 else 250000, lp, cb.ctypes.data)
         assert np.array_equal(ca, cb) and np.array_equal(a, b)
+
+
+def _level_grid():
+    import test_level_fuzz
+    return test_level_fuzz.GRID
+
+
+@pytest.mark.parametrize("levels", _level_grid(), ids=lambda g: ",".join(f"{k}={v:g}" for k, v in g.items()))
+def test_level_grid_on_hostile_iq(ref, levels):
+    """The level fuzz's grid (tests/test_level_fuzz.py: level_limit, min_level, min_snr one at a time, in envelope and
+    magnitude mode, and three combined points) on every hostile-IQ family: the GPU suite judges the kernels by the
+    oracle alone there, so the oracle must equal the reference at every point -- packages, widths, events, stages."""
+    import hostile_iq
+    import test_front_fuzz
+    devs = ref.registered()
+    o = orc.Oracle(store_bitbuffers=False, store_stages=True)
+    o.add_devices(devs)
+    ref.set_levels(**levels)
+    o.set_levels(**levels)
+    try:
+        for name in hostile_iq.FAMILIES:
+            for c in test_front_fuzz.family_cases(name, 0):
+                want = ref.run(c.iq, c.fmt, c.rate, c.freq, c.fpdm)
+                d = helpers.compare_results(want, o.run(c.iq, c.fmt, c.rate, c.freq, c.fpdm), f"oracle, {c}, {levels}")
+                assert not d, "\n".join(d[:12])
+    finally:
+        ref.set_levels()
+        o.close()
