@@ -127,6 +127,8 @@ typedef struct r433b_timing {
     float grab_ms;           /* k_grab of the last r433b_grab_copy() / r433b_grab_tail() (device time, no copy-out) */
     uint32_t chain_folds;       /* chained batches: chunk ends that folded a deferred carrier-estimate log ... */
     uint32_t chain_fm_rebuilds; /* ... and that made the FM filter state exact at the chunk end */
+    float grab_ring_ms;      /* grabbing chains: k_grab_ring of the last chained batch, with the k_grab that saved the
+                                ring bytes it overwrote (device time) */
 } r433b_timing;
 
 int r433b_create(int cuda_device, r433b_ctx **out);
@@ -186,7 +188,8 @@ int r433b_process(r433b_ctx *ctx, r433b_batch const *batch);
      the uncut file's sample_file_pos.  fetch, dispatch*, analyze, digests and gates work on a chained batch unchanged.
    - While any slot is inside a file, the sample format, rate, centre frequency (and so FPDM), block size, levels,
      FM low-pass and whether FM is on (which follows from the devices) must not change: R433B_ESTATE.  A batch whose
-     n_streams differs from the chain's returns R433B_EINVAL.  r433b_grab_plan() on a chained batch returns R433B_ESTATE.
+     n_streams differs from the chain's returns R433B_EINVAL.  r433b_grab_plan() and r433b_grab_tail() on a batch of
+     a chain that does not grab (r433b_chain_grab below) return R433B_ESTATE.
    - A chain belongs to the context that created it and owns its device memory: per slot the carried state, the
      pulse-train scratch (19.2 KB) and a copy of both (a batch whose result arenas overflow runs again from it), about
      40 KB per slot.  r433b_destroy() frees the device memory of the context's chains; such a chain only accepts
@@ -199,6 +202,30 @@ void r433b_chain_destroy(r433b_chain *chain);
 int r433b_process_chained(r433b_ctx *ctx, r433b_batch const *batch, r433b_chain *chain, uint8_t const *last);
 /* absolute sample index of the first sample of slot i's chunk in the last chained batch */
 int r433b_chain_base(r433b_chain const *chain, uint32_t stream, uint64_t *first_sample);
+/* The signal grabber on a chain (`rtl_433 -S`, see the grabber below): every slot is its own grabber run, as one
+   rtl_433 process with one receiver is.  For a slot's files, taken in order, the grabs equal those of
+   `rtl_433 -S <mode> -r f1 -r f2 ...`, and those of one unchained batch that holds the files in that order.
+   - Opt-in, in one mode (R433B_GRAB_*) for the chain's life: a frame's decision takes in the events of every call it
+     spans.  Call it while every slot is at a file start (R433B_ESTATE otherwise, and when the chain grabs already).
+   - It allocates one R433B_GRAB_RING (3 MiB) ring per slot on the device, R433B_ENOMEM if that fails: 12.9 GB for
+     4096 slots.  A batch of chunks longer than one block also keeps, until the next chained batch, the older ring
+     bytes its append overwrote that its frames may still read: at most min(chunk, ring) - 1 block per slot.
+   - A slot's run is the used bytes of its chunks in call order, across its files, after load-time conversion (cs8 as
+     cu8, cf32 as cs16).  The ring is never cleared between files; ring bytes the run never wrote read as zeros.
+   - Frames are tracked per slot and per file (reset_sdr_flow()) and carried from one call to the next: a frame may
+     span any number of calls and end at a later block call or at its file's flush.  Its events (modes 2-3) and
+     analyzer verdict (mode 4) are gathered over every call it spans.
+   - After each chained batch, r433b_grab_plan(ctx, res, mode, NULL, ...) lists the grabs whose frames ended in it,
+     slot by slot.  prior must be NULL and mode the chain's (R433B_EINVAL otherwise).  In r433b_grab, stream is the
+     slot; counter is the grab's 1-based ordinal in its slot's run (sg_counter when no name existed: the access() loop
+     is the caller's, one per slot); first_package / n_packages name the frame's packages in this batch (those of
+     earlier batches are known by seq); run_end counts the slot run's bytes.  Modes 2-4 need their dispatch (and
+     r433b_analyze()) per batch, as unchained.  r433b_grab_copy() then works as unchained, until the next chained
+     batch; r433b_grab_tail() returns R433B_ESTATE.
+   - A chained batch on a grabbing chain whose last batch was not planned returns R433B_ESTATE: its frames would be
+     lost.  When appending a batch to the rings fails, the call fails and the chain's rings no longer match its runs:
+     later chained batches and plans of that chain return R433B_ESTATE. */
+int r433b_chain_grab(r433b_chain *chain, int mode);
 
 /* Copy the compact results to host memory owned by the context. */
 int r433b_fetch(r433b_ctx *ctx, r433b_results *out);

@@ -51,6 +51,13 @@ struct HostBuf {
     size_t cap = 0;
 };
 
+// A stream's frame between block calls (src/r_flow.c:345-362): ages of its first and last package, the decoded
+// events and the analyzer verdict of its packages so far.  Zero when no frame is open.
+struct GrabFrame {
+    uint32_t start_ago = 0, end_ago = 0, quality = 0;
+    uint64_t events = 0;
+};
+
 } // namespace
 
 struct r433b_ctx {
@@ -131,9 +138,11 @@ struct r433b_ctx {
     uint64_t grab_prior_bytes = 0;    // of which the device copy of the tail holds the last ones
     std::vector<uint64_t> grab_cum;   // run offset of stream i within the batch (used bytes), n_streams + 1
     DevBuf d_grab_prior, d_grab_segs, d_grab_stage;
-    // the last batch was a chained one (r433b_process_chained): absolute sample index of each stream's first sample
+    // the last batch was a chained one (r433b_process_chained): absolute sample index of each stream's first sample,
+    // and its chain (null once that chain is destroyed)
     bool chained = false;
     std::vector<uint64_t> chain_base;
+    r433b_chain *chain_last = nullptr;
     std::vector<r433b_chain *> chains; // alive: r433b_destroy() frees their device memory and detaches them
 };
 
@@ -161,6 +170,19 @@ struct r433b_chain {
     std::vector<uint64_t> next;    // ... whose next chunk starts at this absolute sample
     std::vector<uint64_t> base;    // first sample of slot i's chunk in the last chained batch
     ChainSettings settings{};
+    // signal grabber (r433b_chain_grab): each slot is its own run with a kGrabRingBytes ring on the device
+    int grab_mode = 0;
+    bool grab_pending = false;     // the last chained batch has not been planned yet
+    bool grab_failed = false;      // appending a batch to the rings failed: they no longer match the runs
+    DevBuf d_ring, d_pre, d_ring_slots;
+    std::vector<uint64_t> run;     // bytes slot i's run has pushed, after the last chained batch ...
+    std::vector<uint64_t> run_c0;  // ... and before it
+    // the ring bytes [pre_lo, min(run_c0, run - ring)) that the last append overwrote but whose frames may still need
+    // them, saved at d_pre + pre_off
+    std::vector<uint64_t> pre_lo, pre_off;
+    std::vector<GrabFrame> frame, frame_next; // per slot, before the last chained batch and after it (its plan)
+    std::vector<uint32_t> counter, counter_next;
+    std::vector<uint8_t> ended;    // the slot's file ended with the last chained batch
 };
 
 struct r433b_pulses {
@@ -170,7 +192,8 @@ struct r433b_pulses {
 namespace {
 void chain_free_device(r433b_chain *ch)
 {
-    for (DevBuf *b : {&ch->d_state, &ch->d_train, &ch->d_state_copy, &ch->d_train_copy, &ch->d_flags, &ch->d_base}) {
+    for (DevBuf *b : {&ch->d_state, &ch->d_train, &ch->d_state_copy, &ch->d_train_copy, &ch->d_flags, &ch->d_base,
+                      &ch->d_ring, &ch->d_pre, &ch->d_ring_slots}) {
         if (b->p) cudaFree(b->p);
         b->p = nullptr;
         b->cap = 0;
@@ -508,6 +531,8 @@ int slice_ranges(r433b_ctx *ctx, std::vector<GroupRange> const &ranges, unsigned
     return R433B_OK;
 }
 
+int chain_grab_append(r433b_ctx *ctx, r433b_chain *ch);
+
 // rtl_433 -r on every stream of the batch; with a chain, stream i is the next chunk of slot i's file (r433b.h)
 int process_iq(r433b_ctx *ctx, r433b_batch const *b, r433b_chain *ch, uint8_t const *last)
 {
@@ -538,6 +563,12 @@ int process_iq(r433b_ctx *ctx, r433b_batch const *b, r433b_chain *ch, uint8_t co
     if (ch) {
         if (ch->ctx != ctx || !last) return fail(ctx, R433B_EINVAL, "r433b_process_chained: chain of another context, or no last[]");
         if (b->n_streams != ch->n) return fail(ctx, R433B_EINVAL, "r433b_process_chained: n_streams differs from the chain's");
+        if (ch->grab_failed)
+            return fail(ctx, R433B_ESTATE, "r433b_process_chained: a batch of this grabbing chain failed while "
+                                           "appending to its rings");
+        if (ch->grab_pending)
+            return fail(ctx, R433B_ESTATE, "r433b_process_chained: the grabbing chain's last batch was not planned "
+                                           "(r433b_grab_plan): its frames would be lost");
         if (std::find(ch->open.begin(), ch->open.end(), 1) != ch->open.end() && !(settings == ch->settings))
             return fail(ctx, R433B_ESTATE, "r433b_process_chained: format, rate, frequency, block size, levels or FM "
                                            "settings changed while a file of the chain is open");
@@ -552,6 +583,7 @@ int process_iq(r433b_ctx *ctx, r433b_batch const *b, r433b_chain *ch, uint8_t co
     CU(cudaSetDevice(ctx->device));
     ctx->processed = ctx->fetched = false;
     ctx->chained = false;
+    ctx->chain_last = nullptr;
     ctx->pulse_mode = false;
     ctx->batch = *b;
     ctx->batch.sample_format = (uint32_t)SS; // the host replay only needs the sample size (dm_state.sample_size)
@@ -570,6 +602,7 @@ int process_iq(r433b_ctx *ctx, r433b_batch const *b, r433b_chain *ch, uint8_t co
     ctx->grabs.clear();
     ctx->grab_planned = false;
     ctx->timing.grab_ms = 0;
+    ctx->timing.grab_ring_ms = 0;
     uint64_t const total_bytes = b->n_streams ? b->offsets[b->n_streams] / in_div : 0;
     uint64_t used_bytes = 0;
     for (uint64_t v : ctx->lengths) used_bytes += v;
@@ -681,8 +714,10 @@ int process_iq(r433b_ctx *ctx, r433b_batch const *b, r433b_chain *ch, uint8_t co
         CU(cudaMemcpyAsync(ch->d_train.p, ch->d_train_copy.p, b->n_streams * kTrainInts * sizeof(int), cudaMemcpyDeviceToDevice, st));
         return R433B_OK;
     };
-    auto finish_chain = [&]() {
-        if (!ch) return;
+    // the batch has succeeded: the chain moves on, and a grabbing chain appends the chunks to its rings (once, also
+    // after a run that was repeated)
+    auto finish_chain = [&]() -> int {
+        if (!ch) return R433B_OK;
         for (uint32_t i = 0; i < b->n_streams; ++i) {
             ch->open[i] = last[i] ? 0 : 1;
             ch->next[i] = last[i] ? 0 : base[i] + ctx->lengths[i] / SS;
@@ -691,6 +726,10 @@ int process_iq(r433b_ctx *ctx, r433b_batch const *b, r433b_chain *ch, uint8_t co
         ch->settings = settings;
         ctx->chained = true;
         ctx->chain_base = base;
+        ctx->chain_last = ch;
+        if (!ch->grab_mode) return R433B_OK;
+        for (uint32_t i = 0; i < b->n_streams; ++i) ch->ended[i] = last[i] ? 1 : 0;
+        return chain_grab_append(ctx, ch);
     };
 
     uint64_t max_samples = 0;
@@ -904,8 +943,7 @@ int process_iq(r433b_ctx *ctx, r433b_batch const *b, r433b_chain *ch, uint8_t co
             ctx->timing.detect_launches = (unsigned)G;
             ctx->timing.slice_launches = (unsigned)G;
             ctx->processed = true;
-            finish_chain();
-            return R433B_OK;
+            return finish_chain();
         }
         // an arena was too small: grow from what the device counted and redo sequentially below
         unsigned cnt[4];
@@ -985,8 +1023,7 @@ int process_iq(r433b_ctx *ctx, r433b_batch const *b, r433b_chain *ch, uint8_t co
     ctx->timing.d2h_ms = 0;
     ctx->timing.detect_launches = detect_launches;
     ctx->processed = true;
-    finish_chain();
-    return R433B_OK;
+    return finish_chain();
 }
 
 } // namespace
@@ -1022,6 +1059,7 @@ void r433b_chain_destroy(r433b_chain *ch)
     if (!ch) return;
     if (r433b_ctx *ctx = ch->ctx) {
         ctx->chains.erase(std::remove(ctx->chains.begin(), ctx->chains.end(), ch), ctx->chains.end());
+        if (ctx->chain_last == ch) ctx->chain_last = nullptr;
         cudaSetDevice(ctx->device);
         chain_free_device(ch);
     }
@@ -1032,6 +1070,46 @@ int r433b_process_chained(r433b_ctx *ctx, r433b_batch const *b, r433b_chain *cha
 {
     if (!chain || !chain->ctx) return fail(ctx, R433B_EINVAL, "r433b_process_chained: no chain, or its context is gone");
     return process_iq(ctx, b, chain, last);
+}
+
+int r433b_chain_grab(r433b_chain *chain, int mode)
+{
+    if (!chain || !chain->ctx) return R433B_EINVAL;
+    r433b_ctx *ctx = chain->ctx;
+    if (mode < R433B_GRAB_ALL || mode > R433B_GRAB_UNDECODED) return fail(ctx, R433B_EINVAL, "grab mode must be 1 .. 4");
+    if (chain->grab_mode) return fail(ctx, R433B_ESTATE, "r433b_chain_grab: the chain grabs already, in a fixed mode");
+    if (std::find(chain->open.begin(), chain->open.end(), 1) != chain->open.end())
+        return fail(ctx, R433B_ESTATE, "r433b_chain_grab while a file of the chain is open");
+    CU(cudaSetDevice(ctx->device));
+    size_t const n = chain->n;
+    try { // host state first: a failure past this point has only device memory to give back
+
+        chain->run.assign(n, 0);
+        chain->run_c0.assign(n, 0);
+        chain->pre_lo.assign(n, 0);
+        chain->pre_off.assign(n, 0);
+        chain->frame.assign(n, GrabFrame{});
+        chain->frame_next.assign(n, GrabFrame{});
+        chain->counter.assign(n, 1); // samp_grab_create()
+        chain->counter_next.assign(n, 1);
+        chain->ended.assign(n, 0);
+    } catch (std::exception const &) {
+        return fail(ctx, R433B_ENOMEM, "r433b_chain_grab: out of host memory");
+    }
+    cudaError_t e = cudaMalloc(&chain->d_ring.p, n * kGrabRingBytes);
+    if (e != cudaSuccess) {
+        chain->d_ring = DevBuf{};
+        return fail(ctx, R433B_ENOMEM, "r433b_chain_grab: cudaMalloc of the rings", e);
+    }
+    chain->d_ring.cap = n * kGrabRingBytes;
+    if (int r = dev_reserve(ctx, chain->d_ring_slots, n * sizeof(GrabRingSlot))) {
+        cudaFree(chain->d_ring.p);
+        chain->d_ring = DevBuf{};
+        return r;
+    }
+    chain->grab_mode = mode;
+    chain->grab_pending = false;
+    return R433B_OK;
 }
 
 int r433b_chain_base(r433b_chain const *chain, uint32_t stream, uint64_t *first_sample)
@@ -1782,32 +1860,231 @@ void grab_segments(r433b_ctx const *ctx, int64_t a, int64_t b, uint64_t &dst, st
     }
 }
 
+// Slot s's run byte range [a, b) on a grabbing chain after its last batch, as segments: negative positions were never
+// written (zero); the ring holds the newest kGrabRingBytes (split at its wrap); older bytes of the chunk come from the
+// batch, older ones before it from the bytes the append overwrote (saved at d_pre).
+void chain_grab_segments(r433b_ctx const *ctx, r433b_chain const *ch, uint32_t s, int64_t a, int64_t b, uint64_t &dst,
+        std::vector<GrabSeg> &segs)
+{
+    int64_t const S = kGrabRingBytes, c0 = (int64_t)ch->run_c0[s], ring_lo = (int64_t)ch->run[s] - S;
+    while (a < b) {
+        GrabSeg g{};
+        g.dst = dst;
+        int64_t e;
+        if (a < 0) {
+            e = std::min<int64_t>(b, 0);
+            g.kind = kGrabZero;
+        } else if (a >= ring_lo) {
+            int64_t const pos = a % S;
+            e = std::min<int64_t>(b, a - pos + S);
+            g.kind = kGrabRing;
+            g.src = (uint64_t)(uintptr_t)ch->d_ring.p + (uint64_t)s * kGrabRingBytes + (uint64_t)pos;
+        } else if (a >= c0) {
+            e = std::min<int64_t>(b, ring_lo);
+            g.kind = kGrabBatch;
+            g.src = ctx->offsets[s] + (uint64_t)(a - c0);
+        } else {
+            e = std::min<int64_t>(std::min<int64_t>(b, c0), ring_lo);
+            g.kind = kGrabPrior;
+            g.src = ch->pre_off[s] + (uint64_t)(a - (int64_t)ch->pre_lo[s]);
+        }
+        g.len = (uint64_t)(e - a);
+        segs.push_back(g);
+        dst += g.len;
+        a = e;
+    }
+}
+
+// k_grab over `segs` (covering [0, total)) into `out` (device, total rounded up to kGrabSpan)
+int grab_launch(r433b_ctx *ctx, std::vector<GrabSeg> const &segs, uint64_t total, uint8_t const *prior, void *out)
+{
+    cudaStream_t const st = 0;
+    if (int r = dev_reserve(ctx, ctx->d_grab_segs, segs.size() * sizeof(GrabSeg))) return r;
+    CU(cudaMemcpyAsync(ctx->d_grab_segs.p, segs.data(), segs.size() * sizeof(GrabSeg), cudaMemcpyHostToDevice, st));
+    GrabParams gp{};
+    gp.batch = ctx->grab_src;
+    gp.prior = prior;
+    gp.segs = (GrabSeg const *)ctx->d_grab_segs.p;
+    gp.n_segs = (unsigned)segs.size();
+    gp.flip = ctx->grab_flip;
+    gp.total = total;
+    gp.out = (uint4 *)out;
+    uint64_t const warps = (total + kGrabSpan - 1) / kGrabSpan;
+    unsigned const grid = (unsigned)((warps * 32 + kGrabThreads - 1) / kGrabThreads);
+    R4_LAUNCH(k_grab, grid, kGrabThreads, 0, st, gp);
+    CU(cudaGetLastError());
+    return R433B_OK;
+}
+
 // k_grab over `segs` (covering [0, total)) into the staging buffer, then one copy to `out`
 int grab_gather(r433b_ctx *ctx, std::vector<GrabSeg> const &segs, uint64_t total, uint8_t *out)
 {
     if (!total) return R433B_OK;
     cudaStream_t const st = 0;
     uint64_t const staged = (total + kGrabSpan - 1) / kGrabSpan * kGrabSpan;
-    if (int r = dev_reserve(ctx, ctx->d_grab_segs, segs.size() * sizeof(GrabSeg))) return r;
     if (int r = dev_reserve(ctx, ctx->d_grab_stage, staged)) return r;
-    CU(cudaMemcpyAsync(ctx->d_grab_segs.p, segs.data(), segs.size() * sizeof(GrabSeg), cudaMemcpyHostToDevice, st));
-    GrabParams gp{};
-    gp.batch = ctx->grab_src;
-    gp.prior = (uint8_t const *)ctx->d_grab_prior.p;
-    gp.segs = (GrabSeg const *)ctx->d_grab_segs.p;
-    gp.n_segs = (unsigned)segs.size();
-    gp.flip = ctx->grab_flip;
-    gp.total = total;
-    gp.out = (uint4 *)ctx->d_grab_stage.p;
-    uint64_t const warps = staged / kGrabSpan;
-    unsigned const grid = (unsigned)((warps * 32 + kGrabThreads - 1) / kGrabThreads);
+    void const *prior = ctx->chained ? ctx->chain_last->d_pre.p : ctx->d_grab_prior.p;
     CU(cudaEventRecord(ctx->ev[0], st));
-    R4_LAUNCH(k_grab, grid, kGrabThreads, 0, st, gp);
-    CU(cudaGetLastError());
+    if (int r = grab_launch(ctx, segs, total, (uint8_t const *)prior, ctx->d_grab_stage.p)) return r;
     CU(cudaEventRecord(ctx->ev[1], st));
     CU(cudaMemcpy(out, ctx->d_grab_stage.p, total, cudaMemcpyDeviceToHost));
     cudaEventElapsedTime(&ctx->timing.grab_ms, ctx->ev[0], ctx->ev[1]);
     return R433B_OK;
+}
+
+static_assert(kGrabRingBytes == R433B_GRAB_RING, "k_grab_ring's ring size");
+
+// After a grabbing chain's batch: save the ring bytes the append overwrites that the batch's frames may still read
+// (k_grab), then append every slot's chunk to its ring (k_grab_ring).  A frame that ends in this batch ends at a block
+// call, so it reads its slot's run from the end of the chunk's first block minus the ring size on.
+int chain_grab_append_launch(r433b_ctx *ctx, r433b_chain *ch)
+{
+    try {
+        cudaStream_t const st = 0;
+        int64_t const S = kGrabRingBytes, B = ctx->batch.block_bytes;
+        uint32_t const n = ch->n;
+        std::vector<GrabSeg> segs;
+        std::vector<GrabRingSlot> slots(n);
+        std::vector<uint64_t> pre_lo(n), pre_off(n);
+        uint64_t pre = 0, max_words = 0;
+        for (uint32_t s = 0; s < n; ++s) {
+            int64_t const L = (int64_t)ctx->lengths[s], c0 = (int64_t)ch->run[s], c1 = c0 + L;
+            int64_t const lo = std::max<int64_t>(0, c0 + std::min(B, L) - S), hi = std::min(c0, c1 - S);
+            pre_lo[s] = (uint64_t)lo;
+            pre_off[s] = pre;
+            for (int64_t a = lo; a < hi;) { // the ring bytes of [lo, hi), split at the wrap
+                int64_t const pos = a % S, e = std::min(hi, a - pos + S);
+                GrabSeg g{};
+                g.dst = pre;
+                g.src = (uint64_t)(uintptr_t)ch->d_ring.p + (uint64_t)s * kGrabRingBytes + (uint64_t)pos;
+                g.len = (uint64_t)(e - a);
+                g.kind = kGrabRing;
+                segs.push_back(g);
+                pre += g.len;
+                a = e;
+            }
+            int64_t const m = std::min(L, S);
+            slots[s].src = ctx->offsets[s] + (uint64_t)(L - m);
+            slots[s].n = (unsigned)m;
+            slots[s].w0 = (unsigned)((c1 - m) % S);
+            max_words = std::max<uint64_t>(max_words, std::min<uint64_t>(((c1 - m) % 16 + m + 15) / 16, S / 16));
+        }
+        CU(cudaEventRecord(ctx->ev[0], st));
+        if (pre) {
+            if (int r = dev_reserve(ctx, ch->d_pre, (pre + kGrabSpan - 1) / kGrabSpan * kGrabSpan)) return r;
+            if (int r = grab_launch(ctx, segs, pre, nullptr, ch->d_pre.p)) return r;
+        }
+        if (max_words) {
+            CU(cudaMemcpyAsync(ch->d_ring_slots.p, slots.data(), n * sizeof(GrabRingSlot), cudaMemcpyHostToDevice, st));
+            GrabRingParams rp{};
+            rp.batch = ctx->grab_src;
+            rp.rings = (uint8_t *)ch->d_ring.p;
+            rp.slots = (GrabRingSlot const *)ch->d_ring_slots.p;
+            uint64_t const per_cta = kGrabThreads / 32 * (kGrabSpan / 16);
+            rp.ctas = (unsigned)((max_words + per_cta - 1) / per_cta);
+            rp.flip = ctx->grab_flip;
+            R4_LAUNCH(k_grab_ring, n * rp.ctas, kGrabThreads, 0, st, rp);
+            CU(cudaGetLastError());
+        }
+        CU(cudaEventRecord(ctx->ev[1], st));
+        CU(cudaEventSynchronize(ctx->ev[1]));
+        cudaEventElapsedTime(&ctx->timing.grab_ring_ms, ctx->ev[0], ctx->ev[1]);
+        // the rings hold the batch: the slots' runs move on
+        for (uint32_t s = 0; s < n; ++s) {
+            ch->run_c0[s] = ch->run[s];
+            ch->run[s] += ctx->lengths[s];
+        }
+        ch->pre_lo.swap(pre_lo);
+        ch->pre_off.swap(pre_off);
+        ch->frame = ch->frame_next;
+        ch->counter = ch->counter_next;
+        ch->grab_pending = true;
+        return R433B_OK;
+    } catch (std::exception const &) { // allocation failures of the host vectors
+        return fail(ctx, R433B_ENOMEM, "r433b_process_chained: out of host memory");
+    }
+}
+
+// A failed append leaves the rings out of step with the runs: the chain then refuses to grab rather than grab wrong
+int chain_grab_append(r433b_ctx *ctx, r433b_chain *ch)
+{
+    int const r = chain_grab_append_launch(ctx, ch);
+    if (r) ch->grab_failed = true;
+    return r;
+}
+
+// The block calls of push_sdr_flow() on stream s (src/rtl_433.c:1797-1854, src/r_flow.c:137-147, :245-362): its
+// blocks from blk0 on, then the flush when its file ends.  `base` is the run's byte count before the stream's first
+// call; f carries the stream's frame in and out, `counter` the run's file counter, k the first package not yet
+// replayed.  The grabs that `mode` takes go to ctx->grabs.
+void grab_replay(r433b_ctx *ctx, r433b_results const *res, int mode, uint32_t s, uint64_t base, uint64_t blk0,
+        bool flush, GrabFrame &f, uint32_t &counter, uint32_t &k)
+{
+    uint32_t const S = R433B_GRAB_RING;
+    uint32_t const SS = ctx->batch.sample_format, B = ctx->batch.block_bytes;
+    r433b_package const *pk = res->packages;
+    uint32_t const n_pk = res->n_packages;
+    uint64_t const L = ctx->lengths[s];
+    uint64_t const n_blocks = (L + B - 1) / B, calls = n_blocks + (flush ? 1 : 0); // call n_blocks is the flush
+    uint32_t first = UINT32_MAX; // the frame's first package in this batch
+    while (k < n_pk && pk[k].stream < s) ++k;
+    for (uint64_t c = 0; c < calls; ++c) {
+        uint64_t const blk = blk0 + c;
+        bool const here = k < n_pk && pk[k].stream == s && (uint64_t)pk[k].block == blk;
+        if (!f.start_ago && !here) { // no frame and no package: nothing but ageing until the next package
+            if (k < n_pk && pk[k].stream == s && (uint64_t)pk[k].block > blk) c = (uint64_t)pk[k].block - blk0 - 1;
+            else break;
+            continue;
+        }
+        uint64_t const len = c < n_blocks ? std::min<uint64_t>(B, L - c * B) : 0;
+        uint32_t const n_samples = (uint32_t)(len / SS);
+        uint64_t const P = base + std::min<uint64_t>(L, c * B + len); // pushed after this call's push
+        if (f.start_ago) f.start_ago += n_samples;
+        if (f.end_ago) f.end_ago += n_samples;
+        for (; k < n_pk && pk[k].stream == s && (uint64_t)pk[k].block == blk; ++k) {
+            if (!f.start_ago) {
+                f.start_ago = pk[k].start_ago;
+                first = k;
+            } else if (first == UINT32_MAX)
+                first = k;
+            f.end_ago = pk[k].end_ago;
+            uint32_t const pe = ctx->p_events[k];
+            f.events += pe;
+            if (mode == R433B_GRAB_UNDECODED && pe == 0) {
+                uint32_t const q = (uint32_t)analysis_check(pk[k].num_pulses, ctx->an[ctx->dev_index[k]]);
+                if (q > f.quality) f.quality = q;
+            }
+        }
+        if (!(f.start_ago && f.end_ago > n_samples)) continue;
+        bool const take = mode == R433B_GRAB_ALL || (mode == R433B_GRAB_UNKNOWN && f.events == 0)
+                || (mode == R433B_GRAB_KNOWN && f.events > 0) || (mode == R433B_GRAB_UNDECODED && f.events == 0 && f.quality > 0);
+        if (take) {
+            // unsigned arithmetic of src/r_flow.c:352-356 and samp_grab_write(), src/samp_grab.c:98-134
+            uint32_t const pad = n_samples / 8;
+            uint32_t const start_padded = f.start_ago + pad, end_padded = f.end_ago - pad;
+            uint32_t const grab_len = start_padded - end_padded;
+            uint32_t bsize = SS * grab_len;
+            bsize += 131072u - bsize % 131072u;
+            uint32_t const sg_len = (uint32_t)std::min<uint64_t>(P, S);
+            if (bsize > sg_len) bsize = sg_len;
+            uint32_t const sg_index = (uint32_t)(P % S);
+            uint32_t end_pos = SS * end_padded;
+            end_pos = sg_index >= end_pos ? sg_index - end_pos : S - end_pos + sg_index;
+            uint64_t const back = ((uint64_t)sg_index + S - end_pos % S) % S; // bytes between window end and newest
+            r433b_grab g{};
+            g.stream = s;
+            g.first_package = first == UINT32_MAX ? k : first;
+            g.n_packages = k - g.first_package;
+            g.grab_len = grab_len;
+            g.bytes = bsize;
+            g.counter = counter++;
+            g.run_end = (int64_t)P - (int64_t)back;
+            ctx->grabs.push_back(g);
+            ctx->grab_newest.push_back((int64_t)P);
+        }
+        f = GrabFrame{};
+        first = UINT32_MAX;
+    }
 }
 
 } // namespace
@@ -1823,9 +2100,15 @@ int r433b_grab_plan(r433b_ctx *ctx, r433b_results const *res, int mode, r433b_gr
         if (prior && prior->pushed && !prior->tail) return fail(ctx, R433B_EINVAL, "prior ring without its tail");
         if (!ctx->fetched) return fail(ctx, R433B_ESTATE, "r433b_grab_plan before r433b_fetch");
         if (ctx->pulse_mode) return fail(ctx, R433B_ESTATE, "a batch of loaded pulse data has no IQ to grab");
-        if (ctx->chained)
-            return fail(ctx, R433B_ESTATE, "the grabber does not run on chained batches: the reference has no ring order "
-                                           "for files that are open at the same time");
+        r433b_chain *const ch = ctx->chained ? ctx->chain_last : nullptr;
+        if (ctx->chained) {
+            if (!ch || !ch->grab_mode)
+                return fail(ctx, R433B_ESTATE, "the chain of this batch does not grab (r433b_chain_grab before its files)");
+            if (ch->grab_failed)
+                return fail(ctx, R433B_ESTATE, "appending this batch to its chain's rings failed");
+            if (prior) return fail(ctx, R433B_EINVAL, "a chained batch's plan takes no prior: the chain holds the rings");
+            if (mode != ch->grab_mode) return fail(ctx, R433B_EINVAL, "grab mode differs from the chain's");
+        }
         if (res->packages != (r433b_package const *)ctx->h_pkgs.p || res->n_packages != ctx->n_pkgs)
             return fail(ctx, R433B_EINVAL, "results are not the context's last fetched batch");
         if (mode != R433B_GRAB_ALL)
@@ -1835,88 +2118,34 @@ int r433b_grab_plan(r433b_ctx *ctx, r433b_results const *res, int mode, r433b_gr
         if (mode == R433B_GRAB_UNDECODED && !ctx->analyzed)
             return fail(ctx, R433B_ESTATE, "grab mode 4 (undecoded) needs r433b_analyze() first");
         CU(cudaSetDevice(ctx->device));
-        uint32_t const S = R433B_GRAB_RING;
-        uint64_t const pushed = prior ? prior->pushed : 0;
-        uint64_t const tail = std::min<uint64_t>(pushed, S);
-        if (int r = dev_reserve(ctx, ctx->d_grab_prior, tail + 16)) return r;
-        if (tail) CU(cudaMemcpy(ctx->d_grab_prior.p, prior->tail, tail, cudaMemcpyHostToDevice));
-        ctx->grab_pushed = pushed;
-        ctx->grab_prior_bytes = tail;
         uint32_t const n_streams = ctx->batch.n_streams;
-        ctx->grab_cum.assign(n_streams + 1, 0);
-        for (uint32_t i = 0; i < n_streams; ++i) ctx->grab_cum[i + 1] = ctx->grab_cum[i] + ctx->lengths[i];
         ctx->grabs.clear();
         ctx->grab_newest.clear();
-
-        // the block calls of push_sdr_flow(), stream by stream (src/rtl_433.c:1797-1854, src/r_flow.c:137-147, :245-362);
-        // the frame state is per file (reset_sdr_flow(), src/r_flow.c:79-97), the ring and the counter are per run
-        uint32_t const SS = ctx->batch.sample_format, B = ctx->batch.block_bytes;
-        uint32_t counter = prior ? prior->counter : 1; // samp_grab_create() starts at 1
-        r433b_package const *pk = res->packages;
         uint32_t k = 0;
-        for (uint32_t s = 0; s < n_streams; ++s) {
-            uint64_t const L = ctx->lengths[s], base = pushed + ctx->grab_cum[s];
-            uint64_t const n_blocks = (L + B - 1) / B; // block n_blocks is the flush
-            uint32_t start_ago = 0, end_ago = 0, quality = 0, first = 0;
-            uint64_t events = 0;
-            while (k < res->n_packages && pk[k].stream < s) ++k;
-            for (uint64_t blk = 0; blk <= n_blocks; ++blk) {
-                bool const here = k < res->n_packages && pk[k].stream == s && (uint64_t)pk[k].block == blk;
-                if (!start_ago && !here) { // no frame and no package: nothing but ageing until the next package
-                    if (k < res->n_packages && pk[k].stream == s && (uint64_t)pk[k].block > blk) blk = (uint64_t)pk[k].block - 1;
-                    else break;
-                    continue;
-                }
-                uint64_t const len = blk < n_blocks ? std::min<uint64_t>(B, L - blk * B) : 0;
-                uint32_t const n_samples = (uint32_t)(len / SS);
-                uint64_t const P = base + std::min<uint64_t>(L, blk * B + len); // pushed after this call's push
-                if (start_ago) start_ago += n_samples;
-                if (end_ago) end_ago += n_samples;
-                uint64_t d_events = 0;
-                for (; k < res->n_packages && pk[k].stream == s && (uint64_t)pk[k].block == blk; ++k) {
-                    if (!start_ago) {
-                        start_ago = pk[k].start_ago;
-                        first = k;
-                    }
-                    end_ago = pk[k].end_ago;
-                    uint32_t const pe = ctx->p_events[k];
-                    d_events += pe;
-                    if (mode == R433B_GRAB_UNDECODED && pe == 0) {
-                        uint32_t const q = (uint32_t)analysis_check(pk[k].num_pulses, ctx->an[ctx->dev_index[k]]);
-                        if (q > quality) quality = q;
-                    }
-                }
-                events += d_events;
-                if (!(start_ago && end_ago > n_samples)) continue;
-                bool const take = mode == R433B_GRAB_ALL || (mode == R433B_GRAB_UNKNOWN && events == 0)
-                        || (mode == R433B_GRAB_KNOWN && events > 0) || (mode == R433B_GRAB_UNDECODED && events == 0 && quality > 0);
-                if (take) {
-                    // unsigned arithmetic of src/r_flow.c:352-356 and samp_grab_write(), src/samp_grab.c:98-134
-                    uint32_t const pad = n_samples / 8;
-                    uint32_t const start_padded = start_ago + pad, end_padded = end_ago - pad;
-                    uint32_t const grab_len = start_padded - end_padded;
-                    uint32_t bsize = SS * grab_len;
-                    bsize += 131072u - bsize % 131072u;
-                    uint32_t const sg_len = (uint32_t)std::min<uint64_t>(P, S);
-                    if (bsize > sg_len) bsize = sg_len;
-                    uint32_t const sg_index = (uint32_t)(P % S);
-                    uint32_t end_pos = SS * end_padded;
-                    end_pos = sg_index >= end_pos ? sg_index - end_pos : S - end_pos + sg_index;
-                    uint64_t const back = ((uint64_t)sg_index + S - end_pos % S) % S; // bytes between window end and newest
-                    r433b_grab g{};
-                    g.stream = s;
-                    g.first_package = first;
-                    g.n_packages = k - first;
-                    g.grab_len = grab_len;
-                    g.bytes = bsize;
-                    g.counter = counter++;
-                    g.run_end = (int64_t)P - (int64_t)back;
-                    ctx->grabs.push_back(g);
-                    ctx->grab_newest.push_back((int64_t)P);
-                }
-                start_ago = 0;
-                events = 0;
-                quality = 0;
+        if (ch) { // every slot is its own run: its frame and counter carry over from the slot's last batch
+            uint32_t const SS = ctx->batch.sample_format, B = ctx->batch.block_bytes;
+            for (uint32_t s = 0; s < n_streams; ++s) {
+                GrabFrame f = ch->frame[s];
+                uint32_t counter = ch->counter[s];
+                grab_replay(ctx, res, mode, s, ch->run_c0[s], ctx->chain_base[s] * SS / B, ch->ended[s], f, counter, k);
+                ch->frame_next[s] = ch->ended[s] ? GrabFrame{} : f; // reset_sdr_flow()
+                ch->counter_next[s] = counter;
+            }
+            ch->grab_pending = false;
+        } else { // one run over the streams in batch order; the frame state is per file (reset_sdr_flow(), src/r_flow.c:79-97)
+            uint32_t const S = R433B_GRAB_RING;
+            uint64_t const pushed = prior ? prior->pushed : 0;
+            uint64_t const tail = std::min<uint64_t>(pushed, S);
+            if (int r = dev_reserve(ctx, ctx->d_grab_prior, tail + 16)) return r;
+            if (tail) CU(cudaMemcpy(ctx->d_grab_prior.p, prior->tail, tail, cudaMemcpyHostToDevice));
+            ctx->grab_pushed = pushed;
+            ctx->grab_prior_bytes = tail;
+            ctx->grab_cum.assign(n_streams + 1, 0);
+            for (uint32_t i = 0; i < n_streams; ++i) ctx->grab_cum[i + 1] = ctx->grab_cum[i] + ctx->lengths[i];
+            uint32_t counter = prior ? prior->counter : 1; // samp_grab_create() starts at 1
+            for (uint32_t s = 0; s < n_streams; ++s) {
+                GrabFrame f{};
+                grab_replay(ctx, res, mode, s, pushed + ctx->grab_cum[s], 0, true, f, counter, k);
             }
         }
         ctx->grab_planned = true;
@@ -1932,21 +2161,26 @@ int r433b_grab_copy(r433b_ctx *ctx, r433b_results const *res, uint32_t first, ui
 {
     try {
         if (!ctx || !res) return fail(ctx, R433B_EINVAL, "null argument");
-        if (!ctx->grab_planned) return fail(ctx, R433B_ESTATE, "r433b_grab_copy before r433b_grab_plan");
+        if (!ctx->grab_planned || (ctx->chained && !ctx->chain_last))
+            return fail(ctx, R433B_ESTATE, "r433b_grab_copy before r433b_grab_plan, or after its chain was destroyed");
         if ((uint64_t)first + count > ctx->grabs.size()) return fail(ctx, R433B_EINVAL, "grab index out of range");
         CU(cudaSetDevice(ctx->device));
         uint64_t dst = 0;
         std::vector<GrabSeg> segs;
         for (uint32_t i = first; i < first + count; ++i) {
             r433b_grab const &g = ctx->grabs[i];
+            auto segments = [&](int64_t a, int64_t b) {
+                if (ctx->chained) chain_grab_segments(ctx, ctx->chain_last, g.stream, a, b, dst, segs);
+                else grab_segments(ctx, a, b, dst, segs);
+            };
             int64_t const lo = g.run_end - (int64_t)g.bytes, hi = g.run_end;
             // positions older than the ring holds read its newest bytes at the same slots (one wrap at most: bytes <= ring)
             int64_t const oldest = ctx->grab_newest[i] - (int64_t)R433B_GRAB_RING;
             if (lo < oldest) {
-                grab_segments(ctx, lo + (int64_t)R433B_GRAB_RING, std::min<int64_t>(hi, oldest) + (int64_t)R433B_GRAB_RING, dst, segs);
-                grab_segments(ctx, oldest, hi, dst, segs);
+                segments(lo + (int64_t)R433B_GRAB_RING, std::min<int64_t>(hi, oldest) + (int64_t)R433B_GRAB_RING);
+                segments(oldest, hi);
             } else
-                grab_segments(ctx, lo, hi, dst, segs);
+                segments(lo, hi);
         }
         if (dst > cap || (dst && !out)) return fail(ctx, R433B_EINVAL, "output buffer smaller than the grabs' bytes");
         return grab_gather(ctx, segs, dst, out);
@@ -1960,6 +2194,7 @@ int r433b_grab_tail(r433b_ctx *ctx, r433b_results const *res, uint8_t *tail, uin
     try {
         if (!ctx || !res || !tail || !pushed) return fail(ctx, R433B_EINVAL, "null argument");
         if (!ctx->grab_planned) return fail(ctx, R433B_ESTATE, "r433b_grab_tail before r433b_grab_plan");
+        if (ctx->chained) return fail(ctx, R433B_ESTATE, "a chained batch's rings stay in its chain: no r433b_grab_tail");
         CU(cudaSetDevice(ctx->device));
         int64_t const end = (int64_t)(ctx->grab_pushed + ctx->grab_cum.back());
         int64_t const begin = std::max<int64_t>(0, end - (int64_t)R433B_GRAB_RING);

@@ -32,7 +32,8 @@ EXPORTS = ["r433b_create", "r433b_destroy", "r433b_last_error", "r433b_set_level
            "r433b_dump_logic_u8", "r433b_set_gates", "r433b_get_gated",
            "r433b_dispatch_r_devices_parallel", "r433b_analyze", "r433b_analysis_get", "r433b_analysis_text",
            "r433b_analysis_events", "r433b_submit", "r433b_wait", "r433b_grab_plan", "r433b_grab_copy", "r433b_grab_tail",
-           "r433b_chain_create", "r433b_chain_destroy", "r433b_process_chained", "r433b_chain_base"]
+           "r433b_chain_create", "r433b_chain_destroy", "r433b_process_chained", "r433b_chain_base",
+           "r433b_chain_grab"]
 
 
 def build(force=False, verbose=False):
@@ -112,7 +113,8 @@ class Timing(C.Structure):
                 ("total_ms", C.c_float), ("detect_launches", C.c_uint32), ("slice_launches", C.c_uint32),
                 ("front_ms", C.c_float), ("front_launches", C.c_uint32), ("front_redone", C.c_uint32),
                 ("front_repairs", C.c_uint32), ("idle_skipped", C.c_uint32), ("idle_rewalks", C.c_uint32),
-                ("grab_ms", C.c_float), ("chain_folds", C.c_uint32), ("chain_fm_rebuilds", C.c_uint32)]
+                ("grab_ms", C.c_float), ("chain_folds", C.c_uint32), ("chain_fm_rebuilds", C.c_uint32),
+                ("grab_ring_ms", C.c_float)]
 
 
 GRAB_ALL, GRAB_UNKNOWN, GRAB_KNOWN, GRAB_UNDECODED = 1, 2, 3, 4
@@ -170,6 +172,7 @@ def load():
     L.r433b_chain_destroy.argtypes = [C.c_void_p]
     L.r433b_process_chained.argtypes = [C.c_void_p, C.POINTER(Batch), C.c_void_p, C.c_void_p]
     L.r433b_chain_base.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint64)]
+    L.r433b_chain_grab.argtypes = [C.c_void_p, C.c_int]
     L.r433b_fetch.argtypes = [C.c_void_p, C.POINTER(Results)]
     L.r433b_get_timing.argtypes = [C.c_void_p, C.POINTER(Timing)]
     L.r433b_get_counts.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
@@ -367,6 +370,11 @@ class Chain:
         if rc:
             raise R433Error(f"r433b_chain_base: {rc}")
         return out.value
+
+    def grab(self, mode):
+        """Grab signals in `mode` (GRAB_*) on every slot, each its own run (include/r433b.h: r433b_chain_grab).  After
+        each chained batch, ctx.grab_plan(mode) lists the grabs whose frames ended in it; ctx.grab_copy gathers them."""
+        self.ctx._check(self.L.r433b_chain_grab(self.h, mode))
 
 
 class Context:
