@@ -2,6 +2,7 @@
 // result fetch, and the CPU-side replay that feeds events to decoders in the reference's order.
 // There is no CPU implementation of the DSP here: every sample goes through k_detect/k_slice2.
 #include <algorithm>
+#include <array>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -73,8 +74,6 @@ struct r433b_ctx {
     r433b_batch batch{};
     std::vector<uint64_t> offsets, lengths; // lengths[i] = bytes of stream i in use
     bool processed = false, fetched = false;
-    unsigned fpdm = 0;
-    int enable_fm = 0;
     int n_sms = 132;        // cudaDevAttrMultiProcessorCount of `device`
     int spoil_front = 0; // R433B_SPOIL_FRONT=1|2|3: k_front starts from wrong guesses (tests of the redo / repair paths)
     // R433B_TEST_CAPS=pkg,pool,arena: initial package / pulse-pool / event-arena caps in place of the defaults (0 keeps
@@ -478,7 +477,7 @@ void launch_slice(r433b_ctx *ctx, GroupRange *range, unsigned n_pkgs, unsigned r
     q.pairs = (r433b_pair *)ctx->d_pairs.p;
     q.arena = (uint8_t *)ctx->d_arena.p;
     q.arena_cap = ctx->arena_cap;
-    q.cursor = (unsigned long long *)ctx->d_cursor.p;
+    q.cursor = (SliceCursor *)ctx->d_cursor.p;
     q.stage = (uint32_t *)ctx->d_stage.p;
     unsigned const bgrid = (unsigned)ctx->n_sms * 2;
     R4_LAUNCH(k_bucket_count, bgrid, kBucketThreads, 0, st, range, pkgs, n_pkgs, n_devs, ss.hist);
@@ -495,7 +494,7 @@ void launch_slice(r433b_ctx *ctx, GroupRange *range, unsigned n_pkgs, unsigned r
 int slice_ranges(r433b_ctx *ctx, std::vector<GroupRange> const &ranges, unsigned n_pkgs, size_t pool_entries, cudaStream_t st)
 {
     unsigned const n_devs = (unsigned)ctx->devs.size();
-    unsigned long long cursor[4] = {0, 0, 0, 0};
+    SliceCursor cur{};
     ctx->timing.slice_launches = 0;
     CU(cudaEventRecord(ctx->ev[2], st));
     if (n_pkgs && n_devs) {
@@ -515,51 +514,58 @@ int slice_ranges(r433b_ctx *ctx, std::vector<GroupRange> const &ranges, unsigned
                 CU(cudaGetLastError());
                 ctx->timing.slice_launches++;
             }
-            CU(cudaMemcpyAsync(cursor, ctx->d_cursor.p, sizeof(cursor), cudaMemcpyDeviceToHost, st));
+            CU(cudaMemcpyAsync(&cur, ctx->d_cursor.p, sizeof(cur), cudaMemcpyDeviceToHost, st));
             CU(cudaStreamSynchronize(st));
-            if (!cursor[2]) break;
-            ctx->arena_cap = (size_t)cursor[0] + (1u << 20);
+            if (!cur.overflow) break;
+            ctx->arena_cap = (size_t)cur.bytes + (1u << 20);
             if (attempt == 2) return fail(ctx, R433B_EOVERFLOW, "event arena overflow");
         }
     }
     CU(cudaEventRecord(ctx->ev[3], st));
     CU(cudaEventSynchronize(ctx->ev[3]));
     cudaEventElapsedTime(&ctx->timing.slice_ms, ctx->ev[2], ctx->ev[3]);
-    ctx->event_bytes = cursor[0];
-    ctx->n_events = cursor[1];
-    ctx->n_gated = cursor[3];
+    ctx->event_bytes = cur.bytes;
+    ctx->n_events = cur.events;
+    ctx->n_gated = cur.gated;
     return R433B_OK;
 }
 
 int chain_grab_append(r433b_ctx *ctx, r433b_chain *ch);
 
-// rtl_433 -r on every stream of the batch; with a chain, stream i is the next chunk of slot i's file (r433b.h)
-int process_iq(r433b_ctx *ctx, r433b_batch const *b, r433b_chain *ch, uint8_t const *last)
+// What process_iq() derives from a batch's arguments
+struct Shape {
+    bool cf32;       // cf32 becomes cs16 on the device before anything else (src/rtl_433.c:1811-1825): from there on
+    unsigned in_div; // offsets, lengths and byte counts are those of the cs16 stream (the input's / in_div)
+    int SS;          // bytes per IQ sample; cs8 is cu8 after the load-time +128
+    ChainSettings settings;
+    uint64_t total_bytes, used_bytes, max_samples; // the last two of the lengths in use (adopt_batch)
+};
+
+// The batch's arguments, and the chain's if it has one.  Changes nothing in the context but the error string.
+int check_batch(r433b_ctx *ctx, r433b_batch const *b, r433b_chain const *ch, uint8_t const *last, Shape &s)
 {
     if (!ctx || !b || !b->offsets || (b->n_streams && !b->data)) return fail(ctx, R433B_EINVAL, "null argument");
     if (b->sample_format != R433B_FMT_CU8 && b->sample_format != R433B_FMT_CS16 && b->sample_format != R433B_FMT_CS8
             && b->sample_format != R433B_FMT_CF32)
         return fail(ctx, R433B_EINVAL, "sample_format must be R433B_FMT_CU8, _CS8, _CS16 or _CF32");
-    // cf32 becomes cs16 on the device before anything else (src/rtl_433.c:1811-1825): from here on
-    // offsets, lengths and byte counts are those of the cs16 stream (half the cf32 ones)
-    bool const cf32 = b->sample_format == R433B_FMT_CF32;
-    unsigned const in_div = cf32 ? 2 : 1;
+    s.cf32 = b->sample_format == R433B_FMT_CF32;
+    s.in_div = s.cf32 ? 2 : 1;
     if (b->samp_rate == 0) return fail(ctx, R433B_EINVAL, "samp_rate is 0");
-    int const SS = (int)(b->sample_format & 0xff); // bytes per IQ sample; cs8 is cu8 after the load-time +128
-    uint32_t block_bytes = b->block_bytes ? b->block_bytes : 262144u;
-    int const T = kTile;
-    if (block_bytes % (uint32_t)(T * SS) != 0) return fail(ctx, R433B_EINVAL, "block_bytes must be a multiple of 2048 samples (4096 bytes of cu8, 8192 of cs16)");
+    s.SS = (int)(b->sample_format & 0xff);
+    uint32_t const block_bytes = b->block_bytes ? b->block_bytes : 262144u;
+    if (block_bytes % (uint32_t)(kTile * s.SS) != 0) return fail(ctx, R433B_EINVAL, "block_bytes must be a multiple of 2048 samples (4096 bytes of cu8, 8192 of cs16)");
     for (uint32_t i = 0; i <= b->n_streams; ++i) {
-        if (b->offsets[i] % (16 * in_div)) return fail(ctx, R433B_EINVAL, "stream offsets must be multiples of 16 bytes (32 for cf32)");
+        if (b->offsets[i] % (16 * s.in_div)) return fail(ctx, R433B_EINVAL, "stream offsets must be multiples of 16 bytes (32 for cf32)");
         if (i && b->offsets[i] < b->offsets[i - 1]) return fail(ctx, R433B_EINVAL, "offsets not ascending");
     }
+    s.total_bytes = b->n_streams ? b->offsets[b->n_streams] / s.in_div : 0;
     int enable_fm = 0;
     for (auto const &d : ctx->devs)
         if (d.modulation >= 16) enable_fm = 1;
     // src/rtl_433.c:1094-1102 and :1515-1522
     unsigned const fpdm = b->fpdm_mode == R433B_FPDM_AUTO ? (b->center_frequency > 800000000u ? 1u : 0u) : b->fpdm_mode;
-    ChainSettings const settings{b->sample_format, b->samp_rate, b->center_frequency, fpdm, block_bytes, ctx->use_mag, enable_fm,
-                                 ctx->level_limit, ctx->min_level, ctx->min_snr, ctx->fm_low_pass};
+    s.settings = ChainSettings{b->sample_format, b->samp_rate, b->center_frequency, fpdm, block_bytes, ctx->use_mag, enable_fm,
+                               ctx->level_limit, ctx->min_level, ctx->min_snr, ctx->fm_low_pass};
     if (ch) {
         if (ch->ctx != ctx || !last) return fail(ctx, R433B_EINVAL, "r433b_process_chained: chain of another context, or no last[]");
         if (b->n_streams != ch->n) return fail(ctx, R433B_EINVAL, "r433b_process_chained: n_streams differs from the chain's");
@@ -569,63 +575,63 @@ int process_iq(r433b_ctx *ctx, r433b_batch const *b, r433b_chain *ch, uint8_t co
         if (ch->grab_pending)
             return fail(ctx, R433B_ESTATE, "r433b_process_chained: the grabbing chain's last batch was not planned "
                                            "(r433b_grab_plan): its frames would be lost");
-        if (std::find(ch->open.begin(), ch->open.end(), 1) != ch->open.end() && !(settings == ch->settings))
+        if (std::find(ch->open.begin(), ch->open.end(), 1) != ch->open.end() && !(s.settings == ch->settings))
             return fail(ctx, R433B_ESTATE, "r433b_process_chained: format, rate, frequency, block size, levels or FM "
                                            "settings changed while a file of the chain is open");
         // a chunk that the file goes on behind is whole blocks: the next one starts on a block boundary
         for (uint32_t i = 0; i < b->n_streams; ++i) {
             uint64_t const in_bytes = b->lengths ? b->lengths[i] : b->offsets[i + 1] - b->offsets[i];
-            if (!last[i] && in_bytes % ((uint64_t)block_bytes * in_div))
+            if (!last[i] && in_bytes % ((uint64_t)block_bytes * s.in_div))
                 return fail(ctx, R433B_EINVAL, "r433b_process_chained: a chunk that is not its file's last must be whole "
                                                "blocks (block_bytes, 2 x block_bytes of cf32 input)");
         }
     }
-    CU(cudaSetDevice(ctx->device));
+    return R433B_OK;
+}
+
+// The batch becomes the context's last one (the host replay reads it), and the results of the one before are gone
+int adopt_batch(r433b_ctx *ctx, r433b_batch const *b, Shape &s)
+{
     ctx->processed = ctx->fetched = false;
-    ctx->chained = false;
+    ctx->chained = ctx->pulse_mode = false;
     ctx->chain_last = nullptr;
-    ctx->pulse_mode = false;
     ctx->batch = *b;
-    ctx->batch.sample_format = (uint32_t)SS; // the host replay only needs the sample size (dm_state.sample_size)
-    ctx->batch.block_bytes = block_bytes;
+    ctx->batch.sample_format = (uint32_t)s.SS; // the host replay only needs the sample size (dm_state.sample_size)
+    ctx->batch.block_bytes = s.settings.block_bytes;
     ctx->offsets.assign(b->offsets, b->offsets + b->n_streams + 1);
-    for (auto &v : ctx->offsets) v /= in_div;
+    for (auto &v : ctx->offsets) v /= s.in_div;
     ctx->batch.offsets = ctx->offsets.data();
     ctx->lengths.resize(b->n_streams);
+    s.used_bytes = s.max_samples = 0;
     for (uint32_t i = 0; i < b->n_streams; ++i) {
         uint64_t gap = b->offsets[i + 1] - b->offsets[i];
         ctx->lengths[i] = b->lengths ? b->lengths[i] : gap;
         if (ctx->lengths[i] > gap) return fail(ctx, R433B_EINVAL, "lengths[i] exceeds the gap to the next offset");
-        if (cf32) ctx->lengths[i] = ctx->lengths[i] / 8 * 4; // whole IQ pairs of floats -> cs16 bytes
+        if (s.cf32) ctx->lengths[i] = ctx->lengths[i] / 8 * 4; // whole IQ pairs of floats -> cs16 bytes
+        s.used_bytes += ctx->lengths[i];
+        s.max_samples = std::max<uint64_t>(s.max_samples, ctx->lengths[i] / s.SS);
     }
     ctx->batch.lengths = ctx->lengths.data();
     ctx->grabs.clear();
     ctx->grab_planned = false;
-    ctx->timing.grab_ms = 0;
-    ctx->timing.grab_ring_ms = 0;
-    uint64_t const total_bytes = b->n_streams ? b->offsets[b->n_streams] / in_div : 0;
-    uint64_t used_bytes = 0;
-    for (uint64_t v : ctx->lengths) used_bytes += v;
-    uint32_t const n_devs = (uint32_t)ctx->devs.size();
-
-    ctx->fpdm = fpdm;
-    ctx->enable_fm = enable_fm;
-
-    cudaStream_t const st = 0;
+    ctx->timing.grab_ms = ctx->timing.grab_ring_ms = 0;
     ctx->d2h_done = false;
+    return R433B_OK;
+}
 
-    // ---- device buffers and launch parameters (no data moved yet) -----------------------
-    uint8_t const *d_in;
-    if (b->data_on_device && !cf32) {
-        d_in = (uint8_t const *)b->data;
-    } else {
-        if (int r = dev_reserve(ctx, ctx->d_data, total_bytes + 64)) return r;
+// The device buffers of the batch (no data moved yet) and the detector's launch parameters, into a zeroed `dp`
+int prepare_detect(r433b_ctx *ctx, r433b_batch const *b, Shape const &s, DetectParams &dp)
+{
+    int const SS = s.SS, T = kTile;
+    uint8_t const *d_in = (uint8_t const *)b->data;
+    if (!b->data_on_device || s.cf32) {
+        if (int r = dev_reserve(ctx, ctx->d_data, s.total_bytes + 64)) return r;
         d_in = (uint8_t const *)ctx->d_data.p;
     }
     ctx->grab_src = d_in; // cf32 is grabbed as the cs16 it was converted to
     ctx->grab_flip = dp_flip_of(b->sample_format);
-    if (cf32 && !b->data_on_device)
-        if (int r = dev_reserve(ctx, ctx->d_raw, 2 * total_bytes + 64)) return r;
+    if (s.cf32 && !b->data_on_device)
+        if (int r = dev_reserve(ctx, ctx->d_raw, 2 * s.total_bytes + 64)) return r;
     if (int r = dev_reserve(ctx, ctx->d_offsets, (b->n_streams + 1) * sizeof(uint64_t))) return r;
     CU(cudaMemcpy(ctx->d_offsets.p, ctx->offsets.data(), (b->n_streams + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice));
     if (int r = dev_reserve(ctx, ctx->d_lengths, std::max<size_t>(1, b->n_streams) * sizeof(uint64_t))) return r;
@@ -646,384 +652,387 @@ int process_iq(r433b_ctx *ctx, r433b_batch const *b, r433b_chain *ch, uint8_t co
     if (int r = dev_reserve(ctx, ctx->d_amoff, (b->n_streams + 1) * sizeof(uint64_t))) return r;
     CU(cudaMemcpy(ctx->d_amoff.p, ctx->am_offsets.data(), (b->n_streams + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice));
     if (b->want_stages)
-        if (int r = dev_reserve(ctx, ctx->d_fm, total_bytes / SS * sizeof(int16_t) + 16)) return r;
+        if (int r = dev_reserve(ctx, ctx->d_fm, s.total_bytes / SS * sizeof(int16_t) + 16)) return r;
 
-    DetectParams dp{};
     dp.data = d_in;
     dp.offsets = (unsigned long long const *)ctx->d_offsets.p;
     dp.lengths = (unsigned long long const *)ctx->d_lengths.p;
-    dp.n_streams = b->n_streams;
-    dp.stream0 = 0;
-    dp.stream_end = b->n_streams;
-    dp.sample_begin = 0;
+    dp.n_streams = dp.stream_end = b->n_streams;
     dp.sample_end = ~0ull;
     dp.first_chunk = 1;
-    dp.state = nullptr;
     dp.use_mag = ctx->use_mag;
     dp.flip = dp_flip_of(b->sample_format);
-    dp.enable_fm = ctx->enable_fm;
-    dp.fpdm = (int)ctx->fpdm;
+    dp.enable_fm = s.settings.enable_fm;
+    dp.fpdm = (int)s.settings.fpdm;
     dp.rate = b->samp_rate;
-    dp.block_samples = block_bytes / SS;
+    dp.block_samples = s.settings.block_bytes / SS;
     dp.lv = ctx->lv;
     dp.lpf_a1 = ((int)(0.85408 * 32768)) >> 1; // src/baseband.c:151-152
     dp.lpf_b0 = ((int)(0.07296 * 32768)) >> 1;
-    dp.fm_a1 = dp.fm_b0 = 0;
     dp.wrap_free = 1;
-    if (ctx->enable_fm) {
-        float lp = ctx->fm_low_pass != 0.0f ? ctx->fm_low_pass : ctx->fpdm ? 0.2f : 0.1f; // src/r_flow.c:204
+    if (dp.enable_fm) {
+        float lp = ctx->fm_low_pass != 0.0f ? ctx->fm_low_pass : dp.fpdm ? 0.2f : 0.1f; // src/r_flow.c:204
         fm_coeffs(SS == 4, b->samp_rate, lp, dp.fm_a1, dp.fm_b0);
         long long unity = SS == 2 ? 16384ll : (1ll << 30);
         dp.wrap_free = dp.fm_a1 >= 0 && dp.fm_b0 >= 0 && (long long)dp.fm_a1 + 2ll * dp.fm_b0 <= unity;
     }
     dp.train_scratch = (int *)ctx->d_train.p;
     dp.log_scratch = (unsigned *)ctx->d_log.p;
-    dp.counters = (unsigned *)ctx->d_counters.p;
+    dp.counters = (DetectCounters *)ctx->d_counters.p;
     dp.am_offsets = (unsigned long long const *)ctx->d_amoff.p;
     dp.am = (int16_t *)ctx->d_am.p;
     dp.chunks = (ChunkInfo const *)ctx->d_chunks.p;
     dp.tile_info = (TileInfo const *)ctx->d_tiles.p;
     dp.fm_out = b->want_stages ? (int16_t *)ctx->d_fm.p : nullptr;
+    return R433B_OK;
+}
 
-    // a chained batch: the chain's state and pulse trains, which slots continue a file, which files end, where each
-    // chunk lies in its file.  The state is copied first, so that a run that has to be repeated starts from it again.
-    std::vector<uint64_t> base;
-    if (ch && b->n_streams) {
-        size_t const n = b->n_streams;
-        std::vector<uint8_t> flags(2 * n);
-        base.resize(n);
-        for (size_t i = 0; i < n; ++i) {
-            flags[i] = ch->open[i];
-            flags[n + i] = last[i] ? 1 : 0;
-            base[i] = ch->open[i] ? ch->next[i] : 0;
-        }
-        CU(cudaMemcpy(ch->d_flags.p, flags.data(), 2 * n, cudaMemcpyHostToDevice));
-        CU(cudaMemcpy(ch->d_base.p, base.data(), n * sizeof(uint64_t), cudaMemcpyHostToDevice));
-        CU(cudaMemcpyAsync(ch->d_state_copy.p, ch->d_state.p, n * sizeof(StreamState), cudaMemcpyDeviceToDevice, st));
-        CU(cudaMemcpyAsync(ch->d_train_copy.p, ch->d_train.p, n * kTrainInts * sizeof(int), cudaMemcpyDeviceToDevice, st));
-        dp.state = (StreamState *)ch->d_state.p;
-        dp.cont = (unsigned char const *)ch->d_flags.p;
-        dp.last = (unsigned char const *)ch->d_flags.p + n;
-        dp.base = (unsigned long long const *)ch->d_base.p;
-        dp.train_scratch = (int *)ch->d_train.p;
+int bind_detector_arenas(r433b_ctx *ctx, DetectParams &dp)
+{
+    if (int r = dev_reserve(ctx, ctx->d_pkgs, ctx->pkg_cap * sizeof(r433b_package))) return r;
+    if (int r = dev_reserve(ctx, ctx->d_ppool, ctx->pool_cap * sizeof(int))) return r;
+    if (int r = dev_reserve(ctx, ctx->d_gpool, ctx->pool_cap * sizeof(int))) return r;
+    dp.pkgs = (r433b_package *)ctx->d_pkgs.p;
+    dp.pkg_cap = (unsigned)std::min<size_t>(ctx->pkg_cap, 0xffffffffu);
+    dp.pulse_pool = (int *)ctx->d_ppool.p;
+    dp.gap_pool = (int *)ctx->d_gpool.p;
+    dp.pool_cap = (unsigned)std::min<size_t>(ctx->pool_cap, 0xffffffffu);
+    return R433B_OK;
+}
+
+// A chained batch: the chain's state and pulse trains, which slots continue a file, which files end, where each chunk
+// lies in its file (chain_base).  The state is copied first, so that a run that has to be repeated starts from it again.
+int chain_begin(r433b_ctx *ctx, r433b_chain *ch, uint8_t const *last, DetectParams &dp)
+{
+    if (!ch) return R433B_OK;
+    size_t const n = ch->n;
+    std::vector<uint8_t> flags(2 * n);
+    ctx->chain_base.resize(n);
+    for (size_t i = 0; i < n; ++i) {
+        flags[i] = ch->open[i];
+        flags[n + i] = last[i] ? 1 : 0;
+        ctx->chain_base[i] = ch->open[i] ? ch->next[i] : 0;
     }
-    bool detect_ran = false; // a chained batch that runs again restores the chain's state first
-    auto restore_chain = [&]() -> int {
-        if (!ch || !detect_ran || !b->n_streams) return R433B_OK;
-        CU(cudaMemcpyAsync(ch->d_state.p, ch->d_state_copy.p, b->n_streams * sizeof(StreamState), cudaMemcpyDeviceToDevice, st));
-        CU(cudaMemcpyAsync(ch->d_train.p, ch->d_train_copy.p, b->n_streams * kTrainInts * sizeof(int), cudaMemcpyDeviceToDevice, st));
-        return R433B_OK;
-    };
-    // the batch has succeeded: the chain moves on, and a grabbing chain appends the chunks to its rings (once, also
-    // after a run that was repeated)
-    auto finish_chain = [&]() -> int {
-        if (!ch) return R433B_OK;
-        for (uint32_t i = 0; i < b->n_streams; ++i) {
-            ch->open[i] = last[i] ? 0 : 1;
-            ch->next[i] = last[i] ? 0 : base[i] + ctx->lengths[i] / SS;
-        }
-        ch->base = base;
-        ch->settings = settings;
-        ctx->chained = true;
-        ctx->chain_base = base;
-        ctx->chain_last = ch;
-        if (!ch->grab_mode) return R433B_OK;
-        for (uint32_t i = 0; i < b->n_streams; ++i) ch->ended[i] = last[i] ? 1 : 0;
-        return chain_grab_append(ctx, ch);
-    };
+    CU(cudaMemcpy(ch->d_flags.p, flags.data(), 2 * n, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(ch->d_base.p, ctx->chain_base.data(), n * sizeof(uint64_t), cudaMemcpyHostToDevice));
+    CU(cudaMemcpyAsync(ch->d_state_copy.p, ch->d_state.p, n * sizeof(StreamState), cudaMemcpyDeviceToDevice, 0));
+    CU(cudaMemcpyAsync(ch->d_train_copy.p, ch->d_train.p, n * kTrainInts * sizeof(int), cudaMemcpyDeviceToDevice, 0));
+    dp.state = (StreamState *)ch->d_state.p;
+    dp.cont = (unsigned char const *)ch->d_flags.p;
+    dp.last = (unsigned char const *)ch->d_flags.p + n;
+    dp.base = (unsigned long long const *)ch->d_base.p;
+    dp.train_scratch = (int *)ch->d_train.p;
+    return R433B_OK;
+}
 
-    uint64_t max_samples = 0;
-    for (uint32_t i = 0; i < b->n_streams; ++i) max_samples = std::max<uint64_t>(max_samples, ctx->lengths[i] / SS);
-    // k_front over the tiles [sample_begin, sample_end) of every stream, then the walk over the same range
-    auto launch_detect = [&](DetectParams const &q, cudaStream_t s, cudaEvent_t after_front) {
-        unsigned n = q.stream_end - q.stream0;
-        if (!n) return;
-        uint64_t const t_end = (std::min<uint64_t>(q.sample_end, max_samples) + T - 1) / T, t_begin = q.sample_begin / T;
-        if (t_end > t_begin) {
-            FrontParams fp{};
-            fp.data = q.data;
-            fp.offsets = q.offsets;
-            fp.lengths = q.lengths;
-            fp.am_offsets = q.am_offsets;
-            fp.n_streams = q.n_streams;
-            fp.tile_begin = t_begin;
-            fp.tiles = (unsigned)(t_end - t_begin);
-            fp.use_mag = q.use_mag;
-            fp.flip = q.flip;
-            fp.block_samples = q.block_samples;
-            fp.a1 = q.lpf_a1;
-            fp.b0 = q.lpf_b0;
-            fp.am = q.am;
-            fp.chunks = (ChunkInfo *)ctx->d_chunks.p;
-            fp.tile_info = (TileInfo *)ctx->d_tiles.p;
-            fp.counters = q.counters;
-            fp.spoil = ctx->spoil_front;
-            fp.state = q.state;
-            fp.cont = q.first_chunk ? q.cont : nullptr;
-            uint64_t const warps = (uint64_t)q.n_streams * fp.tiles;
-            unsigned const fgrid = (unsigned)((warps + kFrontWarps - 1) / kFrontWarps);
-            void (*ffn)(FrontParams) = SS == 2 ? k_front<2> : k_front<4>;
-            size_t const fsm = (size_t)kFrontWarps * (SS == 2 ? FrontStage<2>::kBytes : FrontStage<4>::kBytes);
-            R4_LAUNCH(ffn, fgrid, kFrontWarps * 32, fsm, s, fp);
-        }
-        cudaEventRecord(after_front, s);
-        unsigned grid = (n + kDetectWarps - 1) / kDetectWarps;
-        size_t sm = (size_t)kDetectWarps * sizeof(WarpSmem);
-        void (*kfn)(DetectParams) = SS == 2 ? k_detect<2> : k_detect<4>;
-        R4_LAUNCH(kfn, grid, kDetectWarps * 32, sm, s, q);
-    };
+// The batch has succeeded: the chain moves on, and a grabbing chain appends the chunks to its rings (once, also after a
+// run that was repeated)
+int chain_finish(r433b_ctx *ctx, r433b_chain *ch, uint8_t const *last, Shape const &s)
+{
+    if (!ch) return R433B_OK;
+    for (uint32_t i = 0; i < ch->n; ++i) {
+        ch->open[i] = last[i] ? 0 : 1;
+        ch->next[i] = last[i] ? 0 : ctx->chain_base[i] + ctx->lengths[i] / s.SS;
+    }
+    ch->base = ctx->chain_base;
+    ch->settings = s.settings;
+    ctx->chained = true;
+    ctx->chain_last = ch;
+    if (!ch->grab_mode) return R433B_OK;
+    for (uint32_t i = 0; i < ch->n; ++i) ch->ended[i] = last[i] ? 1 : 0;
+    return chain_grab_append(ctx, ch);
+}
 
-    // slicer parameters: per device, scaled to this batch's sample rate on the host
-    if (int r = upload_slicer_tables(ctx, std::vector<uint32_t>{b->samp_rate}, st)) return r;
+// k_front over the tiles [sample_begin, sample_end) of every stream, then the walk over the same range
+void launch_detect(r433b_ctx *ctx, DetectParams const &q, Shape const &s, cudaStream_t st, cudaEvent_t after_front)
+{
+    int const SS = s.SS, T = kTile;
+    uint64_t const t_end = (std::min<uint64_t>(q.sample_end, s.max_samples) + T - 1) / T, t_begin = q.sample_begin / T;
+    if (t_end > t_begin) {
+        FrontParams fp{};
+        fp.data = q.data;
+        fp.offsets = q.offsets;
+        fp.lengths = q.lengths;
+        fp.am_offsets = q.am_offsets;
+        fp.n_streams = q.n_streams;
+        fp.tile_begin = t_begin;
+        fp.tiles = (unsigned)(t_end - t_begin);
+        fp.use_mag = q.use_mag;
+        fp.flip = q.flip;
+        fp.block_samples = q.block_samples;
+        fp.a1 = q.lpf_a1;
+        fp.b0 = q.lpf_b0;
+        fp.am = q.am;
+        fp.chunks = (ChunkInfo *)ctx->d_chunks.p;
+        fp.tile_info = (TileInfo *)ctx->d_tiles.p;
+        fp.counters = q.counters;
+        fp.spoil = ctx->spoil_front;
+        fp.state = q.state;
+        fp.cont = q.first_chunk ? q.cont : nullptr;
+        uint64_t const warps = (uint64_t)q.n_streams * fp.tiles;
+        unsigned const fgrid = (unsigned)((warps + kFrontWarps - 1) / kFrontWarps);
+        void (*ffn)(FrontParams) = SS == 2 ? k_front<2> : k_front<4>;
+        size_t const fsm = (size_t)kFrontWarps * (SS == 2 ? FrontStage<2>::kBytes : FrontStage<4>::kBytes);
+        R4_LAUNCH(ffn, fgrid, kFrontWarps * 32, fsm, st, fp);
+    }
+    cudaEventRecord(after_front, st);
+    unsigned grid = (q.n_streams + kDetectWarps - 1) / kDetectWarps;
+    size_t sm = (size_t)kDetectWarps * sizeof(WarpSmem);
+    void (*kfn)(DetectParams) = SS == 2 ? k_detect<2> : k_detect<4>;
+    R4_LAUNCH(kfn, grid, kDetectWarps * 32, sm, st, q);
+}
 
-    size_t const pkg_min = ctx->min_caps[0] ? ctx->min_caps[0] : (size_t)b->n_streams * 16 + 1024;
-    if (ctx->pkg_cap < pkg_min) ctx->pkg_cap = pkg_min;
-    size_t const pool_min = ctx->min_caps[1] ? ctx->min_caps[1] : ctx->pkg_cap * 128;
-    if (ctx->pool_cap < pool_min) ctx->pool_cap = pool_min;
-    size_t const arena_min = ctx->min_caps[2] ? ctx->min_caps[2] : total_bytes / 2 + (1u << 20);
-    if (ctx->arena_cap < arena_min) ctx->arena_cap = arena_min;
+int check_pair_index(r433b_ctx *ctx, uint64_t n_pkgs)
+{
+    if (n_pkgs * ctx->devs.size() <= 0xffffffffull) return R433B_OK;
+    return fail(ctx, R433B_EOVERFLOW, "packages x devices exceeds the 32-bit pair index (r433b_package.first_pair)");
+}
 
+// The result arrays of a range (packages, both pools, pairs, events): buffers and the bytes [lo, hi) of the range
+struct ResultPart { HostBuf &h; DevBuf const &d; size_t lo, hi; };
+std::array<ResultPart, 5> result_parts(r433b_ctx *ctx, GroupRange const &r)
+{
+    size_t const pk = sizeof(r433b_package), pair = ctx->devs.size() * sizeof(r433b_pair);
+    return {{{ctx->h_pkgs, ctx->d_pkgs, r.pkg_begin * pk, r.pkg_end * pk},
+             {ctx->h_ppool, ctx->d_ppool, r.pool_begin * sizeof(int), r.pool_end * sizeof(int)},
+             {ctx->h_gpool, ctx->d_gpool, r.pool_begin * sizeof(int), r.pool_end * sizeof(int)},
+             {ctx->h_pairs, ctx->d_pairs, r.pkg_begin * pair, r.pkg_end * pair},
+             {ctx->h_events, ctx->d_arena, r.arena_begin, r.arena_end}}};
+}
 
-    // ---- pipelined path: host input cut into G TIME SLICES of every stream; the copy-in of slice
-    //      k+1 and the copy-out of finished ranges overlap the kernels of slice k (three streams).
-    //      detect(k) and slice(k) stay on ONE stream: both are issue-bound, running them
-    //      concurrently only makes each slower (measured).  (Cutting by streams instead does not help: a warp needs the same
-    //      wall time for its stream however few other warps run.)  Detector / filter state is
-    //      carried between launches in `StreamState`; results are identical to one launch. ----
+// Device to host: the results of a range, at the same offsets in the pinned buffers
+int copy_results(r433b_ctx *ctx, GroupRange const &r, cudaStream_t st)
+{
+    for (ResultPart const &p : result_parts(ctx, r))
+        if (p.hi > p.lo && p.d.p) CU(cudaMemcpyAsync((char *)p.h.p + p.lo, (char const *)p.d.p + p.lo, p.hi - p.lo, cudaMemcpyDeviceToHost, st));
+    return R433B_OK;
+}
+
+// How many time slices the batch is cut into (1: one launch), of how many samples per stream.  Slices take host input
+// on a uniform stride, one strided copy each; the streams' LENGTHS may differ: the kernels stop at every stream's end.
+int time_slices(r433b_ctx const *ctx, r433b_batch const *b, Shape const &s, uint64_t &slice_samples)
+{
     int G = ctx->pipeline_groups;
     uint64_t stride = b->n_streams ? ctx->offsets[1] - ctx->offsets[0] : 0;
     bool uniform = b->n_streams > 0 && stride > 0;
-    // one strided copy per time slice needs the streams on a uniform stride; their LENGTHS may differ (capture files of
-    // different sizes padded to a common stride): the kernels stop at every stream's own end
     for (uint32_t i = 0; uniform && i < b->n_streams; ++i)
         if (ctx->offsets[i + 1] - ctx->offsets[i] != stride) uniform = false;
     if (G == 0) { // slice size (tools/e2e_sweep.py sweeps it): many slices of >= 128 KiB per stream for cu8 (4096 streams);
                   // cs16 batches (1024 x 4 MiB, FM on: every launch pays the slowest stream's bursts) want >= 512 KiB
-        uint64_t const min_slice = SS == 4 ? (512u << 10) : (128u << 10);
-        G = (total_bytes >= (256ull << 20) && stride >= (1u << 20)) ? (int)std::min<uint64_t>(r433b_ctx::kMaxGroups, stride / min_slice) : 1;
+        uint64_t const min_slice = s.SS == 4 ? (512u << 10) : (128u << 10);
+        G = (s.total_bytes >= (256ull << 20) && stride >= (1u << 20)) ? (int)std::min<uint64_t>(r433b_ctx::kMaxGroups, stride / min_slice) : 1;
     }
     if (b->data_on_device && ctx->pipeline_groups == 0) G = 1; // device input: slices only when asked for
     // stage arrays: k_detect's stage pass makes FM of whole streams, so that batch must be one launch
-    if (b->want_stages || !n_devs || !uniform || cf32) G = 1;
-    uint64_t slice_samples = 0;
+    if (b->want_stages || ctx->devs.empty() || !uniform || s.cf32) G = 1;
+    slice_samples = 0;
     if (G > 1) {
-        uint64_t n_samp = stride / SS;
-        uint64_t unit = (uint64_t)T; // slices only have to be tile aligned: block effects use absolute positions
+        uint64_t n_samp = stride / s.SS;
+        uint64_t unit = (uint64_t)kTile; // slices only have to be tile aligned: block effects use absolute positions
         slice_samples = (n_samp / G + unit - 1) / unit * unit;
         if (slice_samples == 0 || slice_samples >= n_samp) G = 1;
         else G = (int)((n_samp + slice_samples - 1) / slice_samples);
         if (G > r433b_ctx::kMaxGroups) G = 1;
     }
-    if (G > 1) {
-        using clk = std::chrono::steady_clock;
-        auto t_wall0 = clk::now();
-        if (int r = dev_reserve(ctx, ctx->d_pkgs, ctx->pkg_cap * sizeof(r433b_package))) return r;
-        if (int r = dev_reserve(ctx, ctx->d_order, ctx->pkg_cap * sizeof(unsigned))) return r;
-        if (int r = dev_reserve(ctx, ctx->d_ppool, ctx->pool_cap * sizeof(int))) return r;
-        if (int r = dev_reserve(ctx, ctx->d_gpool, ctx->pool_cap * sizeof(int))) return r;
-        if (int r = reserve_sort(ctx, ctx->pkg_cap, ctx->pool_cap, ctx->s_det)) return r;
-        size_t const pair_cap_bytes = ctx->pkg_cap * n_devs * sizeof(r433b_pair);
-        if (int r = dev_reserve(ctx, ctx->d_pairs, pair_cap_bytes)) return r;
-        if (int r = dev_reserve(ctx, ctx->d_arena, ctx->arena_cap)) return r;
-        if (int r = dev_reserve(ctx, ctx->d_ranges, G * sizeof(GroupRange))) return r;
-        if (int r = dev_reserve(ctx, ctx->d_state, (size_t)b->n_streams * sizeof(StreamState))) return r;
-        if (int r = host_reserve(ctx, ctx->h_ranges, G * sizeof(GroupRange))) return r;
-        dp.pkgs = (r433b_package *)ctx->d_pkgs.p;
-        dp.pkg_cap = (unsigned)std::min<size_t>(ctx->pkg_cap, 0xffffffffu);
-        dp.pulse_pool = (int *)ctx->d_ppool.p;
-        dp.gap_pool = (int *)ctx->d_gpool.p;
-        dp.pool_cap = (unsigned)std::min<size_t>(ctx->pool_cap, 0xffffffffu);
-        if (!ch) dp.state = (StreamState *)ctx->d_state.p;
-        detect_ran = true;
-        GroupRange *d_rg = (GroupRange *)ctx->d_ranges.p;
-        GroupRange *h_rg = (GroupRange *)ctx->h_ranges.p;
-        unsigned const *d_cnt = (unsigned const *)ctx->d_counters.p;
-        unsigned long long const *d_cur = (unsigned long long const *)ctx->d_cursor.p;
+    return G;
+}
 
-        // the table uploads above went through the legacy stream from pageable memory: their DMA may still be
-        // in flight when cudaMemcpy returns, and s_det does not synchronise with stream 0 by itself
-        CU(cudaEventRecord(ctx->ev_init, 0));
-        CU(cudaStreamWaitEvent(ctx->s_det, ctx->ev_init, 0));
-        CU(cudaMemsetAsync(ctx->d_counters.p, 0, 64, ctx->s_det));
-        CU(cudaMemsetAsync(ctx->d_cursor.p, 0, 64, ctx->s_det));
-        CU(cudaMemsetAsync(ctx->d_pairs.p, 0, pair_cap_bytes, ctx->s_det));
-        CU(cudaEventRecord(ctx->ev_init, ctx->s_det));
-        for (int g = 0; g < G; ++g) {
-            uint64_t c0 = (uint64_t)g * slice_samples * SS, c1 = std::min<uint64_t>(stride, c0 + slice_samples * SS);
-            // one strided copy: the same byte range of every stream
-            if (!b->data_on_device)
-                CU(cudaMemcpy2DAsync((uint8_t *)ctx->d_data.p + ctx->offsets[0] + c0, stride,
-                        (uint8_t const *)b->data + ctx->offsets[0] + c0, stride, c1 - c0, b->n_streams,
-                        cudaMemcpyHostToDevice, ctx->s_in));
-            CU(cudaEventRecord(ctx->ev_in[g], ctx->s_in));
-            CU(cudaStreamWaitEvent(ctx->s_det, ctx->ev_in[g], 0));
-            R4_LAUNCH(k_mark, 1, 1, 0, ctx->s_det, d_rg + g, 0, d_cnt, d_cur);
-            CU(cudaEventRecord(ctx->ev_t[4 * g + 0], ctx->s_det));
-            DetectParams dg = dp;
-            dg.sample_begin = (uint64_t)g * slice_samples;
-            dg.sample_end = g == G - 1 ? ~0ull : (uint64_t)(g + 1) * slice_samples;
-            dg.first_chunk = g == 0;
-            launch_detect(dg, ctx->s_det, ctx->ev_f[g]);
-            CU(cudaEventRecord(ctx->ev_t[4 * g + 1], ctx->s_det));
-            R4_LAUNCH(k_mark, 1, 1, 0, ctx->s_det, d_rg + g, 1, d_cnt, d_cur);
-            CU(cudaEventRecord(ctx->ev_det[g], ctx->s_det));
-            R4_LAUNCH(k_mark, 1, 1, 0, ctx->s_det, d_rg + g, 2, d_cnt, d_cur);
-            CU(cudaEventRecord(ctx->ev_t[4 * g + 2], ctx->s_det));
-            launch_slice(ctx, d_rg + g, dp.pkg_cap, 0, ctx->s_det);
-            CU(cudaEventRecord(ctx->ev_t[4 * g + 3], ctx->s_det));
-            R4_LAUNCH(k_mark, 1, 1, 0, ctx->s_det, d_rg + g, 3, d_cnt, d_cur);
-            CU(cudaMemcpyAsync(h_rg + g, d_rg + g, sizeof(GroupRange), cudaMemcpyDeviceToHost, ctx->s_det));
-            CU(cudaEventRecord(ctx->ev_slc[g], ctx->s_det));
-        }
-        CU(cudaGetLastError());
-        // copy-out of finished groups while later ones compute; only into host buffers that are
-        // already large enough (they are after the first batch of a given shape)
-        bool overflow = false, d2h_ok = !b->data_on_device; // device input: results stay put until r433b_fetch()
-        for (int g = 0; g < G; ++g) {
-            CU(cudaEventSynchronize(ctx->ev_slc[g]));
-            GroupRange const r = h_rg[g];
-            if (r.overflow) overflow = true;
-            if (overflow) continue;
-            size_t pk_hi = (size_t)r.pkg_end * sizeof(r433b_package), pool_hi = (size_t)r.pool_end * sizeof(int);
-            size_t pair_hi = (size_t)r.pkg_end * n_devs * sizeof(r433b_pair);
-            // the same sizes r433b_fetch() reserves (+16): a buffer that passes here is never reallocated there
-            if (ctx->h_pkgs.cap < pk_hi + 16 || ctx->h_ppool.cap < pool_hi + 16 || ctx->h_gpool.cap < pool_hi + 16
-                    || ctx->h_pairs.cap < pair_hi + 16 || ctx->h_events.cap < r.arena_end + 16)
-                d2h_ok = false;
-            if (!d2h_ok) continue;
-            size_t pk_lo = (size_t)r.pkg_begin * sizeof(r433b_package), pool_lo = (size_t)r.pool_begin * sizeof(int);
-            size_t pair_lo = (size_t)r.pkg_begin * n_devs * sizeof(r433b_pair);
-            cudaStream_t so = ctx->s_out;
-            if (pk_hi > pk_lo) CU(cudaMemcpyAsync((char *)ctx->h_pkgs.p + pk_lo, (char *)ctx->d_pkgs.p + pk_lo, pk_hi - pk_lo, cudaMemcpyDeviceToHost, so));
-            if (pool_hi > pool_lo) {
-                CU(cudaMemcpyAsync((char *)ctx->h_ppool.p + pool_lo, (char *)ctx->d_ppool.p + pool_lo, pool_hi - pool_lo, cudaMemcpyDeviceToHost, so));
-                CU(cudaMemcpyAsync((char *)ctx->h_gpool.p + pool_lo, (char *)ctx->d_gpool.p + pool_lo, pool_hi - pool_lo, cudaMemcpyDeviceToHost, so));
-            }
-            if (pair_hi > pair_lo) CU(cudaMemcpyAsync((char *)ctx->h_pairs.p + pair_lo, (char *)ctx->d_pairs.p + pair_lo, pair_hi - pair_lo, cudaMemcpyDeviceToHost, so));
-            if (r.arena_end > r.arena_begin)
-                CU(cudaMemcpyAsync((char *)ctx->h_events.p + r.arena_begin, (char *)ctx->d_arena.p + r.arena_begin, r.arena_end - r.arena_begin, cudaMemcpyDeviceToHost, so));
-        }
-        CU(cudaStreamSynchronize(ctx->s_out));
-        if (!overflow) {
-            GroupRange const last = h_rg[G - 1];
-            if ((uint64_t)last.pkg_end * n_devs > 0xffffffffull)
-                return fail(ctx, R433B_EOVERFLOW, "packages x devices exceeds the 32-bit pair index (r433b_package.first_pair)");
-            ctx->n_pkgs = last.pkg_end;
-            ctx->pool_used = last.pool_end;
-            ctx->event_bytes = last.arena_end;
-            ctx->n_events = last.events_end;
-            ctx->n_gated = last.gated_end;
-            ctx->n_samples = used_bytes / SS;
-            ctx->d2h_done = d2h_ok;
-            float det = 0, slc = 0, frt = 0;
-            for (int g = 0; g < G; ++g) {
-                float a = 0, c = 0, f = 0;
-                cudaEventElapsedTime(&f, ctx->ev_t[4 * g + 0], ctx->ev_f[g]);
-                cudaEventElapsedTime(&a, ctx->ev_f[g], ctx->ev_t[4 * g + 1]);
-                cudaEventElapsedTime(&c, ctx->ev_t[4 * g + 2], ctx->ev_t[4 * g + 3]);
-                frt += f;
-                det += a;
-                slc += c;
-            }
-            ctx->timing.front_ms = frt;
-            ctx->timing.front_launches = (unsigned)G;
-            unsigned stat[10];
-            CU(cudaMemcpy(stat, ctx->d_counters.p, sizeof(stat), cudaMemcpyDeviceToHost));
-            ctx->timing.front_redone = stat[4];
-            ctx->timing.front_repairs = stat[5];
-            ctx->timing.idle_skipped = stat[6];
-            ctx->timing.idle_rewalks = stat[7];
-            ctx->timing.chain_folds = stat[8];
-            ctx->timing.chain_fm_rebuilds = stat[9];
-            ctx->timing.h2d_ms = 0; // overlapped: only the wall total is meaningful
-            ctx->timing.d2h_ms = 0;
-            ctx->timing.detect_ms = det;
-            ctx->timing.slice_ms = slc;
-            ctx->timing.total_ms = std::chrono::duration<float, std::milli>(clk::now() - t_wall0).count();
-            ctx->timing.detect_launches = (unsigned)G;
-            ctx->timing.slice_launches = (unsigned)G;
-            ctx->processed = true;
-            return finish_chain();
-        }
-        // an arena was too small: grow from what the device counted and redo sequentially below
-        unsigned cnt[4];
-        unsigned long long cur[4];
-        CU(cudaMemcpy(cnt, ctx->d_counters.p, sizeof(cnt), cudaMemcpyDeviceToHost));
-        CU(cudaMemcpy(cur, ctx->d_cursor.p, sizeof(cur), cudaMemcpyDeviceToHost));
-        ctx->pkg_cap = std::max<size_t>(ctx->pkg_cap, (size_t)cnt[0] * 2 + 64);
-        ctx->pool_cap = std::max<size_t>(ctx->pool_cap, (size_t)cnt[1] * 2 + 4096);
-        ctx->arena_cap = std::max<size_t>(ctx->arena_cap, (size_t)cur[0] * 2 + (1u << 20));
+// The time-sliced schedule: the copy-in of slice k+1 and the copy-out of finished ranges overlap the kernels of slice
+// k (three streams).  detect(k) and slice(k) stay on ONE stream: both are issue-bound, running them concurrently only
+// makes each slower (measured).  (Cutting by streams instead does not help: a warp needs the same wall time for its
+// stream however few other warps run.)  Detector / filter state is carried between launches in `StreamState`; results
+// are identical to one launch.  kFellBack: an arena overflowed; the caps have grown, the batch runs again in one launch.
+constexpr int kFellBack = 1;
+int run_time_sliced(r433b_ctx *ctx, r433b_batch const *b, Shape const &s, int G, uint64_t slice_samples, DetectParams &dp, DetectCounters &cnt)
+{
+    using clk = std::chrono::steady_clock;
+    auto t_wall0 = clk::now();
+    int const SS = s.SS;
+    uint32_t const n_devs = (uint32_t)ctx->devs.size();
+    uint64_t const stride = ctx->offsets[1] - ctx->offsets[0];
+    if (int r = bind_detector_arenas(ctx, dp)) return r;
+    if (int r = dev_reserve(ctx, ctx->d_order, ctx->pkg_cap * sizeof(unsigned))) return r;
+    if (int r = reserve_sort(ctx, ctx->pkg_cap, ctx->pool_cap, ctx->s_det)) return r;
+    size_t const pair_cap_bytes = ctx->pkg_cap * n_devs * sizeof(r433b_pair);
+    if (int r = dev_reserve(ctx, ctx->d_pairs, pair_cap_bytes)) return r;
+    if (int r = dev_reserve(ctx, ctx->d_arena, ctx->arena_cap)) return r;
+    if (int r = dev_reserve(ctx, ctx->d_ranges, G * sizeof(GroupRange))) return r;
+    if (int r = dev_reserve(ctx, ctx->d_state, (size_t)b->n_streams * sizeof(StreamState))) return r;
+    if (int r = host_reserve(ctx, ctx->h_ranges, G * sizeof(GroupRange))) return r;
+    if (!dp.state) dp.state = (StreamState *)ctx->d_state.p; // a chain carries its own
+    GroupRange *d_rg = (GroupRange *)ctx->d_ranges.p, *h_rg = (GroupRange *)ctx->h_ranges.p;
+    DetectCounters const *d_cnt = (DetectCounters const *)ctx->d_counters.p;
+    SliceCursor const *d_cur = (SliceCursor const *)ctx->d_cursor.p;
+
+    // the table uploads went through the legacy stream from pageable memory: their DMA may still be in flight when
+    // cudaMemcpy returns, and s_det does not synchronise with stream 0 by itself
+    CU(cudaEventRecord(ctx->ev_init, 0));
+    CU(cudaStreamWaitEvent(ctx->s_det, ctx->ev_init, 0));
+    CU(cudaMemsetAsync(ctx->d_counters.p, 0, 64, ctx->s_det));
+    CU(cudaMemsetAsync(ctx->d_cursor.p, 0, 64, ctx->s_det));
+    CU(cudaMemsetAsync(ctx->d_pairs.p, 0, pair_cap_bytes, ctx->s_det));
+    CU(cudaEventRecord(ctx->ev_init, ctx->s_det));
+    for (int g = 0; g < G; ++g) {
+        uint64_t c0 = (uint64_t)g * slice_samples * SS, c1 = std::min<uint64_t>(stride, c0 + slice_samples * SS);
+        // one strided copy: the same byte range of every stream
+        if (!b->data_on_device)
+            CU(cudaMemcpy2DAsync((uint8_t *)ctx->d_data.p + ctx->offsets[0] + c0, stride,
+                    (uint8_t const *)b->data + ctx->offsets[0] + c0, stride, c1 - c0, b->n_streams,
+                    cudaMemcpyHostToDevice, ctx->s_in));
+        CU(cudaEventRecord(ctx->ev_in[g], ctx->s_in));
+        CU(cudaStreamWaitEvent(ctx->s_det, ctx->ev_in[g], 0));
+        R4_LAUNCH(k_mark, 1, 1, 0, ctx->s_det, d_rg + g, 0, d_cnt, d_cur);
+        CU(cudaEventRecord(ctx->ev_t[4 * g + 0], ctx->s_det));
+        DetectParams dg = dp;
+        dg.sample_begin = (uint64_t)g * slice_samples;
+        dg.sample_end = g == G - 1 ? ~0ull : (uint64_t)(g + 1) * slice_samples;
+        dg.first_chunk = g == 0;
+        launch_detect(ctx, dg, s, ctx->s_det, ctx->ev_f[g]);
+        CU(cudaEventRecord(ctx->ev_t[4 * g + 1], ctx->s_det));
+        R4_LAUNCH(k_mark, 1, 1, 0, ctx->s_det, d_rg + g, 1, d_cnt, d_cur);
+        CU(cudaEventRecord(ctx->ev_det[g], ctx->s_det));
+        R4_LAUNCH(k_mark, 1, 1, 0, ctx->s_det, d_rg + g, 2, d_cnt, d_cur);
+        CU(cudaEventRecord(ctx->ev_t[4 * g + 2], ctx->s_det));
+        launch_slice(ctx, d_rg + g, dp.pkg_cap, 0, ctx->s_det);
+        CU(cudaEventRecord(ctx->ev_t[4 * g + 3], ctx->s_det));
+        R4_LAUNCH(k_mark, 1, 1, 0, ctx->s_det, d_rg + g, 3, d_cnt, d_cur);
+        CU(cudaMemcpyAsync(h_rg + g, d_rg + g, sizeof(GroupRange), cudaMemcpyDeviceToHost, ctx->s_det));
+        CU(cudaEventRecord(ctx->ev_slc[g], ctx->s_det));
     }
+    CU(cudaGetLastError());
+    // copy-out of finished groups while later ones compute; only into host buffers that are
+    // already large enough (they are after the first batch of a given shape)
+    bool overflow = false, d2h_ok = !b->data_on_device; // device input: results stay put until r433b_fetch()
+    for (int g = 0; g < G; ++g) {
+        CU(cudaEventSynchronize(ctx->ev_slc[g]));
+        GroupRange const r = h_rg[g];
+        if (r.overflow) overflow = true;
+        if (overflow) continue;
+        // the same sizes r433b_fetch() reserves (+16): a buffer that passes here is never reallocated there
+        for (ResultPart const &p : result_parts(ctx, r)) d2h_ok = d2h_ok && p.h.cap >= p.hi + 16;
+        if (!d2h_ok) continue;
+        if (int rc = copy_results(ctx, r, ctx->s_out)) return rc;
+    }
+    CU(cudaStreamSynchronize(ctx->s_out));
+    CU(cudaMemcpy(&cnt, ctx->d_counters.p, sizeof(cnt), cudaMemcpyDeviceToHost));
+    if (overflow) { // grow from what the device counted
+        SliceCursor cur;
+        CU(cudaMemcpy(&cur, ctx->d_cursor.p, sizeof(cur), cudaMemcpyDeviceToHost));
+        ctx->pkg_cap = std::max<size_t>(ctx->pkg_cap, (size_t)cnt.pkgs * 2 + 64);
+        ctx->pool_cap = std::max<size_t>(ctx->pool_cap, (size_t)cnt.pool * 2 + 4096);
+        ctx->arena_cap = std::max<size_t>(ctx->arena_cap, (size_t)cur.bytes * 2 + (1u << 20));
+        return kFellBack;
+    }
+    GroupRange const end = h_rg[G - 1];
+    if (int r = check_pair_index(ctx, end.pkg_end)) return r;
+    ctx->n_pkgs = end.pkg_end;
+    ctx->pool_used = end.pool_end;
+    ctx->event_bytes = end.arena_end;
+    ctx->n_events = end.events_end;
+    ctx->n_gated = end.gated_end;
+    ctx->d2h_done = d2h_ok;
+    auto ms = [](cudaEvent_t a, cudaEvent_t b) { float t = 0; cudaEventElapsedTime(&t, a, b); return t; };
+    ctx->timing.front_ms = ctx->timing.detect_ms = ctx->timing.slice_ms = 0;
+    for (int g = 0; g < G; ++g) {
+        ctx->timing.front_ms += ms(ctx->ev_t[4 * g + 0], ctx->ev_f[g]);
+        ctx->timing.detect_ms += ms(ctx->ev_f[g], ctx->ev_t[4 * g + 1]);
+        ctx->timing.slice_ms += ms(ctx->ev_t[4 * g + 2], ctx->ev_t[4 * g + 3]);
+    }
+    ctx->timing.h2d_ms = 0; // overlapped: only the wall total is meaningful
+    ctx->timing.total_ms = std::chrono::duration<float, std::milli>(clk::now() - t_wall0).count();
+    ctx->timing.detect_launches = (unsigned)G;
+    ctx->timing.slice_launches = (unsigned)G;
+    return R433B_OK;
+}
 
-    // ---- sequential path ------------------------------------------------------------------
+// The one-launch schedule on stream 0: copy-in, the detector (again with the arenas grown to what it counted while
+// they overflow), then the slicers over all its packages.  `rerun`: the detector has run on this batch before.
+int run_sequential(r433b_ctx *ctx, r433b_batch const *b, Shape const &s, DetectParams &dp, r433b_chain *ch, bool rerun, DetectCounters &cnt)
+{
+    cudaStream_t const st = 0;
     CU(cudaEventRecord(ctx->ev[0], st));
-    if (cf32 && total_bytes) {
+    if (s.cf32 && s.total_bytes) {
         void const *raw = b->data;
         if (!b->data_on_device) {
-            CU(cudaMemcpyAsync(ctx->d_raw.p, b->data, 2 * total_bytes, cudaMemcpyHostToDevice, st));
+            CU(cudaMemcpyAsync(ctx->d_raw.p, b->data, 2 * s.total_bytes, cudaMemcpyHostToDevice, st));
             raw = ctx->d_raw.p;
         }
-        size_t n4 = (size_t)(2 * total_bytes / 16); // groups of four floats (offsets are multiples of 32 bytes)
+        size_t n4 = (size_t)(2 * s.total_bytes / 16); // groups of four floats (offsets are multiples of 32 bytes)
         R4_LAUNCH(k_cf32_to_cs16, ctx->n_sms * 8, 256, 0, st, (float4 const *)raw, (uint2 *)ctx->d_data.p, n4);
         CU(cudaGetLastError());
-    } else if (!b->data_on_device && total_bytes)
-        CU(cudaMemcpyAsync(ctx->d_data.p, b->data, total_bytes, cudaMemcpyHostToDevice, st));
+    } else if (!b->data_on_device && s.total_bytes)
+        CU(cudaMemcpyAsync(ctx->d_data.p, b->data, s.total_bytes, cudaMemcpyHostToDevice, st));
     CU(cudaEventRecord(ctx->ev[1], st));
 
     unsigned detect_launches = 0;
-    unsigned counters[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
     for (int attempt = 0; attempt < 3; ++attempt) {
-        if (int r = restore_chain()) return r;
-        if (int r = dev_reserve(ctx, ctx->d_pkgs, ctx->pkg_cap * sizeof(r433b_package))) return r;
-        if (int r = dev_reserve(ctx, ctx->d_ppool, ctx->pool_cap * sizeof(int))) return r;
-        if (int r = dev_reserve(ctx, ctx->d_gpool, ctx->pool_cap * sizeof(int))) return r;
-        dp.pkgs = (r433b_package *)ctx->d_pkgs.p;
-        dp.pkg_cap = (unsigned)std::min<size_t>(ctx->pkg_cap, 0xffffffffu);
-        dp.pulse_pool = (int *)ctx->d_ppool.p;
-        dp.gap_pool = (int *)ctx->d_gpool.p;
-        dp.pool_cap = (unsigned)std::min<size_t>(ctx->pool_cap, 0xffffffffu);
+        if (ch && (attempt > 0 || rerun)) { // from the state chain_begin() found
+            CU(cudaMemcpyAsync(ch->d_state.p, ch->d_state_copy.p, ch->n * sizeof(StreamState), cudaMemcpyDeviceToDevice, st));
+            CU(cudaMemcpyAsync(ch->d_train.p, ch->d_train_copy.p, ch->n * kTrainInts * sizeof(int), cudaMemcpyDeviceToDevice, st));
+        }
+        if (int r = bind_detector_arenas(ctx, dp)) return r;
         CU(cudaMemsetAsync(ctx->d_counters.p, 0, 64, st));
         if (b->n_streams) {
-            launch_detect(dp, st, ctx->ev[4]);
+            launch_detect(ctx, dp, s, st, ctx->ev[4]);
             CU(cudaGetLastError());
             detect_launches++;
-            detect_ran = true;
         }
-        CU(cudaMemcpyAsync(counters, ctx->d_counters.p, sizeof(counters), cudaMemcpyDeviceToHost, st));
+        CU(cudaMemcpyAsync(&cnt, ctx->d_counters.p, sizeof(cnt), cudaMemcpyDeviceToHost, st));
         CU(cudaStreamSynchronize(st));
-        if (!counters[2]) break;
+        if (!cnt.overflow) break;
         // arenas were too small: the counters hold the true need
-        ctx->pkg_cap = std::max<size_t>(ctx->pkg_cap, (size_t)counters[0] + 64);
-        ctx->pool_cap = std::max<size_t>(ctx->pool_cap, (size_t)counters[1] + 4096);
+        ctx->pkg_cap = std::max<size_t>(ctx->pkg_cap, (size_t)cnt.pkgs + 64);
+        ctx->pool_cap = std::max<size_t>(ctx->pool_cap, (size_t)cnt.pool + 4096);
         if (attempt == 2) return fail(ctx, R433B_EOVERFLOW, "package arena overflow");
     }
-    if ((uint64_t)counters[0] * n_devs > 0xffffffffull)
-        return fail(ctx, R433B_EOVERFLOW, "packages x devices exceeds the 32-bit pair index (r433b_package.first_pair)");
-    ctx->n_pkgs = counters[0];
-    ctx->pool_used = counters[1];
+    if (int r = check_pair_index(ctx, cnt.pkgs)) return r;
+    ctx->n_pkgs = cnt.pkgs;
+    ctx->pool_used = cnt.pool;
     GroupRange all{};
     all.pkg_end = ctx->n_pkgs;
     if (int r = slice_ranges(ctx, std::vector<GroupRange>{all}, ctx->n_pkgs, ctx->pool_used, st)) return r;
-    ctx->n_samples = used_bytes / SS;
     cudaEventElapsedTime(&ctx->timing.h2d_ms, ctx->ev[0], ctx->ev[1]);
     ctx->timing.front_ms = 0;
-    if (detect_launches) {
-        cudaEventElapsedTime(&ctx->timing.front_ms, ctx->ev[1], ctx->ev[4]);
-        cudaEventElapsedTime(&ctx->timing.detect_ms, ctx->ev[4], ctx->ev[2]);
-    } else
-        cudaEventElapsedTime(&ctx->timing.detect_ms, ctx->ev[1], ctx->ev[2]);
-    ctx->timing.front_launches = detect_launches;
-    ctx->timing.front_redone = counters[4];
-    ctx->timing.front_repairs = counters[5];
-    ctx->timing.idle_skipped = counters[6];
-    ctx->timing.idle_rewalks = counters[7];
-    ctx->timing.chain_folds = counters[8];
-    ctx->timing.chain_fm_rebuilds = counters[9];
+    if (detect_launches) cudaEventElapsedTime(&ctx->timing.front_ms, ctx->ev[1], ctx->ev[4]);
+    cudaEventElapsedTime(&ctx->timing.detect_ms, ctx->ev[detect_launches ? 4 : 1], ctx->ev[2]); // with the counter read-back
     cudaEventElapsedTime(&ctx->timing.total_ms, ctx->ev[0], ctx->ev[3]);
-    ctx->timing.d2h_ms = 0;
     ctx->timing.detect_launches = detect_launches;
+    return R433B_OK;
+}
+
+// rtl_433 -r on every stream of the batch; with a chain, stream i is the next chunk of slot i's file (r433b.h)
+int process_iq(r433b_ctx *ctx, r433b_batch const *b, r433b_chain *ch, uint8_t const *last)
+{
+    Shape s{};
+    if (int r = check_batch(ctx, b, ch, last, s)) return r;
+    CU(cudaSetDevice(ctx->device));
+    if (int r = adopt_batch(ctx, b, s)) return r;
+    DetectParams dp{};
+    if (int r = prepare_detect(ctx, b, s, dp)) return r;
+    if (int r = chain_begin(ctx, ch, last, dp)) return r;
+    // slicer parameters: per device, scaled to this batch's sample rate on the host
+    if (int r = upload_slicer_tables(ctx, std::vector<uint32_t>{b->samp_rate}, 0)) return r;
+    ctx->pkg_cap = std::max<size_t>(ctx->pkg_cap, ctx->min_caps[0] ? ctx->min_caps[0] : (size_t)b->n_streams * 16 + 1024);
+    ctx->pool_cap = std::max<size_t>(ctx->pool_cap, ctx->min_caps[1] ? ctx->min_caps[1] : ctx->pkg_cap * 128);
+    ctx->arena_cap = std::max<size_t>(ctx->arena_cap, ctx->min_caps[2] ? ctx->min_caps[2] : s.total_bytes / 2 + (1u << 20));
+    uint64_t slice_samples;
+    int const G = time_slices(ctx, b, s, slice_samples);
+    DetectCounters cnt{};
+    int r = kFellBack;
+    if (G > 1) r = run_time_sliced(ctx, b, s, G, slice_samples, dp, cnt);
+    if (r == kFellBack) r = run_sequential(ctx, b, s, dp, ch, G > 1, cnt);
+    if (r) return r;
+    ctx->timing.front_redone = cnt.front_redone;
+    ctx->timing.front_repairs = cnt.front_repairs;
+    ctx->timing.idle_skipped = cnt.idle_skipped;
+    ctx->timing.idle_rewalks = cnt.idle_rewalks;
+    ctx->timing.chain_folds = cnt.chain_folds;
+    ctx->timing.chain_fm_rebuilds = cnt.chain_fm_rebuilds;
+    ctx->timing.front_launches = ctx->timing.detect_launches;
+    ctx->timing.d2h_ms = 0; // r433b_fetch()'s, or overlapped
+    ctx->n_samples = s.used_bytes / s.SS;
     ctx->processed = true;
-    return finish_chain();
+    return chain_finish(ctx, ch, last, s);
 }
 
 } // namespace
@@ -1144,23 +1153,15 @@ int r433b_fetch(r433b_ctx *ctx, r433b_results *out)
     CU(cudaSetDevice(ctx->device));
     cudaStream_t const st = 0;
     uint32_t const n_devs = (uint32_t)ctx->devs.size();
-    size_t pk_bytes = (size_t)ctx->n_pkgs * sizeof(r433b_package);
-    size_t pool_bytes = (size_t)ctx->pool_used * sizeof(int);
-    size_t pair_bytes = (size_t)ctx->n_pkgs * n_devs * sizeof(r433b_pair);
+    GroupRange all{};
+    all.pkg_end = ctx->n_pkgs;
+    all.pool_end = ctx->pool_used;
+    all.arena_end = ctx->event_bytes;
     CU(cudaEventRecord(ctx->ev[4], st));
-    if (int r = host_reserve(ctx, ctx->h_pkgs, pk_bytes + 16)) return r;
-    if (int r = host_reserve(ctx, ctx->h_ppool, pool_bytes + 16)) return r;
-    if (int r = host_reserve(ctx, ctx->h_gpool, pool_bytes + 16)) return r;
-    if (int r = host_reserve(ctx, ctx->h_pairs, pair_bytes + 16)) return r;
-    if (int r = host_reserve(ctx, ctx->h_events, ctx->event_bytes + 16)) return r;
+    for (ResultPart const &p : result_parts(ctx, all))
+        if (int r = host_reserve(ctx, p.h, p.hi + 16)) return r;
     if (!ctx->d2h_done) {
-        if (pk_bytes) CU(cudaMemcpyAsync(ctx->h_pkgs.p, ctx->d_pkgs.p, pk_bytes, cudaMemcpyDeviceToHost, st));
-        if (pool_bytes) {
-            CU(cudaMemcpyAsync(ctx->h_ppool.p, ctx->d_ppool.p, pool_bytes, cudaMemcpyDeviceToHost, st));
-            CU(cudaMemcpyAsync(ctx->h_gpool.p, ctx->d_gpool.p, pool_bytes, cudaMemcpyDeviceToHost, st));
-        }
-        if (pair_bytes && ctx->d_pairs.p) CU(cudaMemcpyAsync(ctx->h_pairs.p, ctx->d_pairs.p, pair_bytes, cudaMemcpyDeviceToHost, st));
-        if (ctx->event_bytes) CU(cudaMemcpyAsync(ctx->h_events.p, ctx->d_arena.p, ctx->event_bytes, cudaMemcpyDeviceToHost, st));
+        if (int r = copy_results(ctx, all, st)) return r;
         ctx->d2h_done = true;
     }
     CU(cudaEventRecord(ctx->ev[5], st));
@@ -1554,8 +1555,7 @@ int r433b_process_pulses(r433b_ctx *ctx, r433b_pulses const *ps)
     PulseSet const &set = ps->set;
     uint32_t const n = (uint32_t)set.pk.size();
     uint32_t const n_devs = (uint32_t)ctx->devs.size();
-    if ((uint64_t)n * n_devs > 0xffffffffull)
-        return fail(ctx, R433B_EOVERFLOW, "packages x devices exceeds the 32-bit pair index (r433b_package.first_pair)");
+    if (int r = check_pair_index(ctx, n)) return r;
     ctx->processed = ctx->fetched = false;
     ctx->d2h_done = false;
     ctx->pulse_mode = true;

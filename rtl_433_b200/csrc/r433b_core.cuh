@@ -613,4 +613,25 @@ R4_HD PackageHeader package_header(DetState const &d, int type)
     return h;
 }
 
+// ------------------------------------------------------------- device counters --------
+
+// The detector's words of a batch, zeroed in front of it: k_detect reserves packages and pool entries here, k_front
+// and k_detect count what their shortcuts did (r433b_timing), k_mark reads the totals between pipelined launches
+struct DetectCounters {
+    unsigned pkgs, pool; // packages stored, pool entries reserved
+    unsigned overflow;   // a package or its widths did not fit: the batch runs again with larger arenas
+    unsigned unused;
+    unsigned front_redone, front_repairs, idle_skipped, idle_rewalks, chain_folds, chain_fm_rebuilds;
+};
+
+// The slicers' words of a batch (k_slice2), zeroed in front of it
+struct SliceCursor {
+    unsigned long long bytes;    // event arena bytes reserved
+    unsigned long long events;   // events stored
+    unsigned long long overflow; // an output did not fit the arena: the batch slices again with a larger one
+    unsigned long long gated;    // events dropped by a gate
+};
+
+static_assert(sizeof(DetectCounters) == 40 && sizeof(SliceCursor) == 32, "the counter buffers hold 64 bytes");
+
 } // namespace r433b

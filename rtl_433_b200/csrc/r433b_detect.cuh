@@ -102,7 +102,7 @@ struct WalkConst {
     r433b_package *pkgs;
     int *pulse_pool, *gap_pool;
     unsigned pkg_cap, pool_cap;
-    unsigned *counters;
+    DetectCounters *counters;
     TileInfo const *tiles;       // the stream's tile summaries; nullptr: no tile is skipped (idle_skip)
 };
 
@@ -147,7 +147,7 @@ struct DetectParams {
     unsigned pkg_cap;
     int *pulse_pool, *gap_pool;
     unsigned pool_cap;
-    unsigned *counters; // [0] packages, [1] pool entries, [2] overflow flag, [4..] statistics
+    DetectCounters *counters;
     int16_t *am;               // k_front's output (repaired in place where a tile did not fit its predecessor)
     ChunkInfo const *chunks;   // bounds of every 64-sample chunk of `am`
     TileInfo const *tile_info; // summary of every tile of `am` (as k_front made it: never updated by a repair)
@@ -598,14 +598,14 @@ __device__ R4_NOINLINE void walk_emit(WarpSmem &sm, int type, unsigned long long
     unsigned cnt = h.num_pulses + 1 < (unsigned)kMaxPulses ? h.num_pulses + 1 : (unsigned)kMaxPulses;
     unsigned idx = 0, off = 0;
     if (lane == 0) {
-        idx = atomicAdd(&wc.counters[0], 1u);
-        off = atomicAdd(&wc.counters[1], cnt);
+        idx = atomicAdd(&wc.counters->pkgs, 1u);
+        off = atomicAdd(&wc.counters->pool, cnt);
     }
     idx = __shfl_sync(0xffffffffu, idx, 0);
     off = __shfl_sync(0xffffffffu, off, 0);
     bool fits = idx < wc.pkg_cap && (unsigned long long)off + cnt <= wc.pool_cap;
     if (!fits) {
-        if (lane == 0) atomicOr(&wc.counters[2], 1u);
+        if (lane == 0) atomicOr(&wc.counters->overflow, 1u);
     } else {
         __syncwarp();
         int const *sp = type == 1 ? tr.ook_pulse : tr.fsk_pulse;
@@ -946,7 +946,7 @@ __device__ R4_NOINLINE unsigned long long idle_skip(WarpSmem &sm, int16_t const 
                 sm.ws.d.high = d.high;
                 sm.ws.d.lead_in = d.lead_in;
                 sm.ws.skip_y = y;
-                atomicAdd(&sm.wc.counters[6], (unsigned)((t - t0) / T));
+                atomicAdd(&sm.wc.counters->idle_skipped, (unsigned)((t - t0) / T));
             }
             __syncwarp();
             return t;
@@ -954,7 +954,7 @@ __device__ R4_NOINLINE unsigned long long idle_skip(WarpSmem &sm, int16_t const 
         // not resolved: the run is walked again from t0 (ws.d still holds the exact state there)
         if (lane == 0) {
             sm.ws.rewalk_end = (unsigned)(t / T);
-            atomicAdd(&sm.wc.counters[7], 1u);
+            atomicAdd(&sm.wc.counters->idle_rewalks, 1u);
         }
     }
     if (lane == 0) sm.ws.skip_y = y_am;
@@ -1327,7 +1327,7 @@ __device__ R4_NOINLINE void chunk_end(WarpSmem &sm, StreamState *ss)
     unsigned long long const N = jb.N;
     if (sm.ws.log_n || sm.ws.log_count) {
         walk_f1_fold<SS>(sm);
-        if (lane == 0) atomicAdd(&sm.wc.counters[8], 1u);
+        if (lane == 0) atomicAdd(&sm.wc.counters->chain_folds, 1u);
     }
     if (jb.fm_on && sm.fm_state.pos != N) {
         if (jb.monotone) {
@@ -1338,7 +1338,7 @@ __device__ R4_NOINLINE void chunk_end(WarpSmem &sm, StreamState *ss)
                 fm_window<SS>(jb, sm, w0, N - w0 < (unsigned long long)kFmWin ? (int)(N - w0) : kFmWin);
             }
         }
-        if (lane == 0) atomicAdd(&sm.wc.counters[9], 1u);
+        if (lane == 0) atomicAdd(&sm.wc.counters->chain_fm_rebuilds, 1u);
     }
     int ci, cq;
     iq_at<SS>(jb.src, N - 1, jb.flip, ci, cq);
@@ -1513,7 +1513,7 @@ __global__ void __launch_bounds__(kDetectWarps * 32, kDetectCtasPerSm) k_detect(
                 int const expect = iir16_nowrap(y_am, a1, b0, x0 + xm);
                 if (expect != (int)(int16_t)am16[0]) {
                     am_repair<SS>(sm, src, t0, nv_tile, y_am, xm, a1, b0, p.flip, p.use_mag, am_stream + t0);
-                    if (lane == 0) atomicAdd(&p.counters[5], 1u);
+                    if (lane == 0) atomicAdd(&p.counters->front_repairs, 1u);
                 }
             }
         }

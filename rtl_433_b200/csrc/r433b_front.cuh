@@ -205,7 +205,7 @@ struct FrontParams {
     int16_t *am;
     ChunkInfo *chunks;                    // one per 64 samples of `am`
     TileInfo *tile_info;                  // one per tile of `am`
-    unsigned *counters;                   // [4] chunks done twice
+    DetectCounters *counters;             // front_redone: chunks done twice
     int spoil;                            // tests: 1 = lane 0's guess is made wrong, 2 = every lane's, 3 = lane 0's in every
                                           // 7th tile, 4 = lane 0's in every tile incl. tile 0 of a continued chunk
                                           // (R433B_SPOIL_FRONT)
@@ -431,7 +431,7 @@ __global__ void __launch_bounds__(kFrontWarps * 32, kFrontCtasPerSm) k_front(Fro
         run = lane == f;
         if (run) {
             fixed = true;
-            atomicAdd(&p.counters[4], 1u);
+            atomicAdd(&p.counters->front_redone, 1u);
         }
     }
     __syncwarp();

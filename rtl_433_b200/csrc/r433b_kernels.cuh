@@ -60,23 +60,23 @@ struct GroupRange {
     unsigned count[2], groups[2];
 };
 
-__global__ void k_mark(GroupRange *r, int which, unsigned const *counters, unsigned long long const *cursor)
+__global__ void k_mark(GroupRange *r, int which, DetectCounters const *counters, SliceCursor const *cursor)
 {
     if (which == 0) {
-        r->pkg_begin = counters[0];
-        r->pool_begin = counters[1];
+        r->pkg_begin = counters->pkgs;
+        r->pool_begin = counters->pool;
     } else if (which == 1) {
-        r->pkg_end = counters[0];
-        r->pool_end = counters[1];
-        r->overflow = counters[2];
+        r->pkg_end = counters->pkgs;
+        r->pool_end = counters->pool;
+        r->overflow = counters->overflow;
         r->next = 0;
     } else if (which == 2) {
-        r->arena_begin = cursor[0];
+        r->arena_begin = cursor->bytes;
     } else {
-        r->arena_end = cursor[0];
-        r->events_end = cursor[1];
-        r->gated_end = cursor[3];
-        r->overflow |= (unsigned)cursor[2] << 1;
+        r->arena_end = cursor->bytes;
+        r->events_end = cursor->events;
+        r->gated_end = cursor->gated;
+        r->overflow |= (unsigned)cursor->overflow << 1;
     }
 }
 
@@ -236,8 +236,8 @@ struct SliceParams {
     r433b_pair *pairs;        // n_pkgs * n_devs, pre-zeroed
     uint8_t *arena;
     unsigned long long arena_cap;
-    unsigned long long *cursor; // [0] bytes reserved, [1] events stored, [2] overflow, [3] events dropped by a gate
-    uint32_t *stage;            // kStageWords per thread of the (fixed) grid
+    SliceCursor *cursor;
+    uint32_t *stage;          // kStageWords per thread of the (fixed) grid
 };
 
 constexpr int kSliceThreads = 128;
@@ -311,14 +311,14 @@ __global__ void __launch_bounds__(kSliceThreads, kSliceCtasPerSm) k_slice2(Slice
         }
         unsigned long long wbase = 0;
         if (lane == 0 && total) {
-            wbase = atomicAdd(p.cursor, (unsigned long long)total);
-            atomicAdd(p.cursor + 1, (unsigned long long)evs);
+            wbase = atomicAdd(&p.cursor->bytes, (unsigned long long)total);
+            atomicAdd(&p.cursor->events, (unsigned long long)evs);
         }
-        if (lane == 0 && dropped) atomicAdd(p.cursor + 3, (unsigned long long)dropped);
+        if (lane == 0 && dropped) atomicAdd(&p.cursor->gated, (unsigned long long)dropped);
         wbase = __shfl_sync(0xffffffffu, wbase, 0);
         unsigned long long const off = wbase + incl - bytes;
         bool const fits = off + bytes <= p.arena_cap;
-        if (active && bytes && !fits) atomicOr(p.cursor + 2, 1ull);
+        if (active && bytes && !fits) atomicOr(&p.cursor->overflow, 1ull);
         if (__all_sync(0xffffffffu, bytes <= kStageWords * 4)) {
             // word i of the warp's range [wbase, wbase + total) belongs to the last lane whose output starts at or
             // before i; the lanes take 32 consecutive words, aligned to a 128-byte line, at a time
