@@ -129,6 +129,10 @@ typedef struct r433b_timing {
     uint32_t chain_fm_rebuilds; /* ... and that made the FM filter state exact at the chunk end */
     float grab_ring_ms;      /* grabbing chains: k_grab_ring of the last chained batch, with the k_grab that saved the
                                 ring bytes it overwrote (device time) */
+    uint32_t split_segments; /* segmented replay (r433b_set_split): slots walked in pass 1, 0 when the batch ran unsplit */
+    uint32_t split_rewalks;  /* segments walked again from their predecessor's end state */
+    uint32_t split_rounds;   /* rewalk launches */
+    float split_merge_ms;    /* k_split_merge_scan + k_split_merge (device time) */
 } r433b_timing;
 
 int r433b_create(int cuda_device, r433b_ctx **out);
@@ -143,6 +147,29 @@ int r433b_set_fm_low_pass(r433b_ctx *ctx, float fm_low_pass);
 /* Host-input batches are cut into `groups` runs of streams whose copy-in, kernels and copy-out
    overlap (0 = automatic, 1 = no overlap, <= 16).  Results are identical either way. */
 int r433b_set_pipeline(r433b_ctx *ctx, int groups);
+
+/* Segmented replay: k_detect walks one stream with one warp, so a batch of a few long captures leaves most of the GPU
+   idle.  With splitting on, r433b_process() (and r433b_submit()) cuts each long stream at block boundaries into
+   segments of segment_blocks blocks and walks them on separate warps:
+   - pass 0 walks, as a file start, the warmup_blocks blocks in front of every segment but a stream's first; its end
+     state is the segment's seed (the state the detector would have had the recording begun there);
+   - pass 1 walks every segment, the first from the file start and every other from its seed;
+   - a segment whose seed differs from its predecessor's end state (every field that can still be read: detector,
+     AM and FM filters, carried IQ sample, deferred carrier-estimate log, the open package's trains) is walked again
+     from that end state, in rounds, until every segment has started from the exact state;
+   - the packages of every segment's last walk are merged on the device and sliced once.
+   The results are those of the unsplit batch, bit for bit, whatever the seeds were.
+   - segment_blocks 0 turns splitting off (the default).  R433B_SPLIT_AUTO chooses from the batch: it splits only when
+     the batch has fewer streams than k_detect has resident warps (streams_per_sm x SMs, 32 x 132 on an H100), only
+     streams of at least 4 segments of at least 2 blocks, with segments sized so that the slots number about one per
+     resident warp.
+   - warmup_blocks is 1 .. segment_blocks (R433B_EINVAL otherwise; with R433B_SPLIT_AUTO it is capped to the chosen
+     segment).  A warm-up never reaches in front of its stream's start.
+   - Batches with want_stages, chained batches and batches in which no stream has two segments run unsplit.
+   - Memory on the device, per slot: the state and pulse trains of the walk and of its seed (about 40 KB), plus one
+     rewalk slot per stream.  r433b_timing.split_* report what the schedule did. */
+#define R433B_SPLIT_AUTO 0xffffffffu
+int r433b_set_split(r433b_ctx *ctx, uint32_t segment_blocks, uint32_t warmup_blocks);
 
 /* The registered decoder list in registration order (cfg->demod->r_devs, src/r_api.c:267). */
 int r433b_set_devices(r433b_ctx *ctx, r433b_device const *devs, uint32_t n);

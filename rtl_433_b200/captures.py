@@ -11,6 +11,9 @@
 * `--chunk-mb N` streams every group through a chain (r433b_process_chained): each call reads the next N MiB of
   whole blocks of every file at an offset, so host memory is about (files in the group) x N MiB; the printed
   output is that of the plain run.  It does not combine with `-S`.
+* `--split [N|auto]` walks long files in segments of N blocks on separate warps (r433b_set_split; `auto` sizes them
+  from the batch); the printed output, and the files `-S all` writes, are those of the plain run.  It does not
+  combine with `--chunk-mb`.
 * `-S all [--grab-dir DIR]` is the signal grabber (src/samp_grab.c): every frame's IQ is written to
   `g%03u_%gM_%gk.cu8|.cs16` files as `rtl_433 -S all -r FILES...` writes them.  The grabber's ring runs
   across the files in processing order, which is group order: the files of each (format, rate,
@@ -370,10 +373,11 @@ def _replay_chunked(ctx, batch, chunk_mb, report):
     return reps
 
 
-def replay(specs, protocols=None, cuda_device=0, max_rows=8, out=print, grab_mode=0, grab_dir=".", chunk_mb=0):
+def replay(specs, protocols=None, cuda_device=0, max_rows=8, out=print, grab_mode=0, grab_dir=".", chunk_mb=0, split=0):
     """Run capture files through the GPU path; report packages and slicer output per file.  grab_mode 1 writes
     every frame's IQ to grab_dir (`-S all`).  chunk_mb > 0 streams every group through a chain, chunk_mb MiB of every
-    file per call: the report is the same, host memory stays bounded."""
+    file per call: the report is the same, host memory stays bounded.  split (blocks per segment, or lib.SPLIT_AUTO)
+    walks long files in segments on separate warps: the report is the same, long files finish sooner."""
     table = lib.default_device_table(include_disabled=True)
     if protocols:
         devs = [d for d in table if d["protocol_num"] in set(protocols)]
@@ -383,8 +387,12 @@ def replay(specs, protocols=None, cuda_device=0, max_rows=8, out=print, grab_mod
         raise ValueError("grab modes unknown / known / undecoded need decoder results: use r433b_grab_plan after r433b_dispatch")
     if grab_mode and chunk_mb:
         raise ValueError("the signal grabber does not run on chained batches (-S with --chunk-mb)")
+    if split and chunk_mb:
+        raise ValueError("segmented replay does not run on chained batches (--split with --chunk-mb)")
     ctx = lib.Context(cuda_device)
     ctx.set_devices(devs)
+    if split:
+        ctx.set_split(split)
     grabber = Grabber(grab_dir) if grab_mode else None
     summary = []
     try:
@@ -418,13 +426,25 @@ def main(argv=None):
     ap.add_argument("--grab-dir", default=".", help="directory for the grabbed files (default: the current one)")
     ap.add_argument("--chunk-mb", type=int, default=0, metavar="N",
                     help="stream every file through a chain, N MiB of whole blocks per call (bounded host memory)")
+    ap.add_argument("--split", nargs="?", const="auto", default=None, metavar="N|auto",
+                    help="walk long files in segments of N blocks on separate warps (auto: sized from the batch)")
     a = ap.parse_args(argv)
+    split = 0
+    if a.split is not None:
+        if a.split == "auto":
+            split = lib.SPLIT_AUTO
+        elif a.split.isdigit() and int(a.split) > 0:
+            split = int(a.split)
+        else:
+            ap.error("--split takes a positive number of blocks or 'auto'")
+    if a.split is not None and a.chunk_mb:
+        ap.error("--split does not run with --chunk-mb: segmented replay does not run on chained batches")
     if a.chunk_mb < 0:
         ap.error("--chunk-mb must be positive")
     if a.grab and a.chunk_mb:
         ap.error("-S does not run with --chunk-mb: the signal grabber does not run on chained batches")
     replay(a.files, a.protocols, a.device, grab_mode=lib.GRAB_ALL if a.grab else 0, grab_dir=a.grab_dir,
-           chunk_mb=a.chunk_mb)
+           chunk_mb=a.chunk_mb, split=split)
 
 
 if __name__ == "__main__":

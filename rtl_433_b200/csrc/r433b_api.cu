@@ -23,6 +23,7 @@
 #include "r433b_analyze.cuh"
 #include "r433b_analyze_host.hpp"
 #include "r433b_grab.cuh"
+#include "r433b_split.cuh"
 
 using namespace r433b;
 
@@ -143,6 +144,12 @@ struct r433b_ctx {
     std::vector<uint64_t> chain_base;
     r433b_chain *chain_last = nullptr;
     std::vector<r433b_chain *> chains; // alive: r433b_destroy() frees their device memory and detaches them
+    // segmented replay (r433b_set_split): segment / warm-up blocks (0: off), R433B_SPOIL_SEED=1 (tests of the rewalk
+    // path), the slots' states and trains, their seeds, the rewalk launch's, the launch views and the merge tables
+    uint32_t split_blocks = 0, split_warmup = 1;
+    int spoil_seed = 0;
+    DevBuf d_sp_state, d_sp_train, d_sp_seed, d_sp_seed_train, d_sp_rw_state, d_sp_rw_train;
+    DevBuf d_sp_view, d_sp_flags, d_sp_list, d_sp_eq, d_sp_tab, d_sp_pkgs, d_sp_ppool, d_sp_gpool;
 };
 
 // What must not change while a chain has an open file: everything the carried state depends on
@@ -298,6 +305,7 @@ int r433b_create(int cuda_device, r433b_ctx **out)
     cudaEventCreateWithFlags(&ctx->ev_init, cudaEventDisableTiming);
     ctx->lv = compute_levels(0, 0.0f, -12.1442f, 9.0f);
     if (char const *v = getenv("R433B_SPOIL_FRONT")) ctx->spoil_front = atoi(v);
+    if (char const *v = getenv("R433B_SPOIL_SEED")) ctx->spoil_seed = atoi(v);
     if (char const *v = getenv("R433B_TEST_CAPS")) {
         unsigned long long c[3] = {0, 0, 0};
         sscanf(v, "%llu,%llu,%llu", &c[0], &c[1], &c[2]);
@@ -322,7 +330,10 @@ void r433b_destroy(r433b_ctx *ctx)
                  &ctx->d_counters, &ctx->d_am, &ctx->d_fm, &ctx->d_devparams, &ctx->d_lists, &ctx->d_pairs,
                  &ctx->d_arena, &ctx->d_cursor, &ctx->d_ranges, &ctx->d_state, &ctx->d_lengths, &ctx->d_stage, &ctx->d_raw, &ctx->d_log, &ctx->d_amoff, &ctx->d_chunks, &ctx->d_tiles,
                  &ctx->d_order, &ctx->d_sort, &ctx->d_copy, &ctx->d_an, &ctx->d_an_dev, &ctx->d_an_gap, &ctx->d_an_pairs, &ctx->d_an_arena,
-                 &ctx->d_grab_prior, &ctx->d_grab_segs, &ctx->d_grab_stage})
+                 &ctx->d_grab_prior, &ctx->d_grab_segs, &ctx->d_grab_stage, &ctx->d_sp_state, &ctx->d_sp_train,
+                 &ctx->d_sp_seed, &ctx->d_sp_seed_train, &ctx->d_sp_rw_state, &ctx->d_sp_rw_train, &ctx->d_sp_view,
+                 &ctx->d_sp_flags, &ctx->d_sp_list, &ctx->d_sp_eq, &ctx->d_sp_tab, &ctx->d_sp_pkgs, &ctx->d_sp_ppool,
+                 &ctx->d_sp_gpool})
         if (b->p) cudaFree(b->p);
     for (HostBuf *b : {&ctx->h_pkgs, &ctx->h_ppool, &ctx->h_gpool, &ctx->h_pairs, &ctx->h_events, &ctx->h_ranges})
         if (b->p) cudaFreeHost(b->p);
@@ -365,6 +376,16 @@ int r433b_set_pipeline(r433b_ctx *ctx, int groups)
 {
     if (!ctx || groups < 0 || groups > r433b_ctx::kMaxGroups) return R433B_EINVAL;
     ctx->pipeline_groups = groups;
+    return R433B_OK;
+}
+
+int r433b_set_split(r433b_ctx *ctx, uint32_t segment_blocks, uint32_t warmup_blocks)
+{
+    if (!ctx) return R433B_EINVAL;
+    if (segment_blocks && (warmup_blocks < 1 || (segment_blocks != R433B_SPLIT_AUTO && warmup_blocks > segment_blocks)))
+        return fail(ctx, R433B_EINVAL, "r433b_set_split: warmup_blocks must be 1 .. segment_blocks");
+    ctx->split_blocks = segment_blocks;
+    ctx->split_warmup = segment_blocks ? warmup_blocks : 1;
     return R433B_OK;
 }
 
@@ -945,12 +966,9 @@ int run_time_sliced(r433b_ctx *ctx, r433b_batch const *b, Shape const &s, int G,
     return R433B_OK;
 }
 
-// The one-launch schedule on stream 0: copy-in, the detector (again with the arenas grown to what it counted while
-// they overflow), then the slicers over all its packages.  `rerun`: the detector has run on this batch before.
-int run_sequential(r433b_ctx *ctx, r433b_batch const *b, Shape const &s, DetectParams &dp, r433b_chain *ch, bool rerun, DetectCounters &cnt)
+// The batch's samples to the device whole: host input copied, cf32 converted to cs16
+int copy_in(r433b_ctx *ctx, r433b_batch const *b, Shape const &s, cudaStream_t st)
 {
-    cudaStream_t const st = 0;
-    CU(cudaEventRecord(ctx->ev[0], st));
     if (s.cf32 && s.total_bytes) {
         void const *raw = b->data;
         if (!b->data_on_device) {
@@ -962,6 +980,16 @@ int run_sequential(r433b_ctx *ctx, r433b_batch const *b, Shape const &s, DetectP
         CU(cudaGetLastError());
     } else if (!b->data_on_device && s.total_bytes)
         CU(cudaMemcpyAsync(ctx->d_data.p, b->data, s.total_bytes, cudaMemcpyHostToDevice, st));
+    return R433B_OK;
+}
+
+// The one-launch schedule on stream 0: copy-in, the detector (again with the arenas grown to what it counted while
+// they overflow), then the slicers over all its packages.  `rerun`: the detector has run on this batch before.
+int run_sequential(r433b_ctx *ctx, r433b_batch const *b, Shape const &s, DetectParams &dp, r433b_chain *ch, bool rerun, DetectCounters &cnt)
+{
+    cudaStream_t const st = 0;
+    CU(cudaEventRecord(ctx->ev[0], st));
+    if (int r = copy_in(ctx, b, s, st)) return r;
     CU(cudaEventRecord(ctx->ev[1], st));
 
     unsigned detect_launches = 0;
@@ -1000,6 +1028,318 @@ int run_sequential(r433b_ctx *ctx, r433b_batch const *b, Shape const &s, DetectP
     return R433B_OK;
 }
 
+// ---- segmented replay (r433b_set_split, DESIGN §7c) ---------------------------------------------------------------
+
+// The segments of a batch, stream by stream: segment k is bytes [begin, begin + bytes) of batch stream `stream`
+struct SplitPlan {
+    std::vector<uint32_t> stream, first; // first: the stream's first segment
+    std::vector<uint64_t> begin, bytes;
+    uint64_t warmup = 1;                 // blocks
+};
+
+// false: the batch runs unsplit (splitting off, stage arrays, or no stream of two segments)
+bool plan_split(r433b_ctx const *ctx, r433b_batch const *b, Shape const &s, SplitPlan &p)
+{
+    if (!ctx->split_blocks || b->want_stages || !b->n_streams) return false;
+    uint64_t const bb = s.settings.block_bytes;
+    uint64_t seg = ctx->split_blocks, min_blocks = 0;
+    if (ctx->split_blocks == R433B_SPLIT_AUTO) {
+        uint64_t const warps = (uint64_t)ctx->n_sms * kDetectCtasPerSm * kDetectWarps, n = b->n_streams;
+        if (n >= warps) return false;
+        uint64_t blocks = 0;
+        for (uint64_t i = 0; i < n; ++i) blocks += (ctx->lengths[i] + bb - 1) / bb;
+        seg = std::max<uint64_t>(kSplitMinSegmentBlocks, (blocks + warps - 1) / warps);
+        min_blocks = seg * kSplitMinSegments;
+    }
+    p.warmup = std::min<uint64_t>(ctx->split_warmup, seg);
+    bool any = false;
+    for (uint32_t i = 0; i < b->n_streams; ++i) {
+        uint64_t const len = ctx->lengths[i], blocks = (len + bb - 1) / bb;
+        uint32_t const first = (uint32_t)p.stream.size();
+        bool const split = blocks > seg && blocks >= min_blocks;
+        any = any || split;
+        for (uint64_t b0 = 0; b0 == 0 || (split && b0 < blocks); b0 += seg) {
+            p.stream.push_back(i);
+            p.first.push_back(first);
+            p.begin.push_back(b0 * bb);
+            p.bytes.push_back(split ? std::min(len, (b0 + seg) * bb) - b0 * bb : len);
+        }
+    }
+    return any;
+}
+
+// The streams of one launch of the split schedule: stream i walks bytes [off, off + len) of the batch's data as a chained
+// chunk whose sample 0 is absolute sample `base` of its file, from the state it holds where `cont`, flushing where `last`
+struct SplitLaunch {
+    std::vector<uint64_t> off, len, base;
+    std::vector<uint8_t> cont, last;
+    void add(uint64_t o, uint64_t l, uint64_t b0, bool c, bool e)
+    {
+        off.push_back(o);
+        len.push_back(l);
+        base.push_back(b0);
+        cont.push_back(c ? 1 : 0);
+        last.push_back(e ? 1 : 0);
+    }
+};
+
+// k_front and k_detect over one launch's streams with `state` / `train` as their chain state; the counters are read back
+// into `cnt` (they go on from the launch before)
+int split_launch(r433b_ctx *ctx, DetectParams const &dp, Shape const &s, SplitLaunch const &v, StreamState *state,
+        int *train, DetectCounters &cnt, float &front_ms, float &detect_ms)
+{
+    cudaStream_t const st = 0;
+    size_t const n = v.off.size();
+    if (!n) return R433B_OK;
+    std::vector<uint64_t> view(4 * n + 2); // offsets (n + 1), lengths, AM offsets (n + 1), bases
+    uint64_t *off = view.data(), *len = off + n + 1, *amoff = len + n, *base = amoff + n + 1;
+    Shape sh = s;
+    sh.max_samples = 0;
+    amoff[0] = 0;
+    for (size_t i = 0; i < n; ++i) {
+        off[i] = v.off[i];
+        len[i] = v.len[i];
+        base[i] = v.base[i];
+        amoff[i + 1] = amoff[i] + (v.len[i] / s.SS + kTile - 1) / kTile * kTile;
+        sh.max_samples = std::max<uint64_t>(sh.max_samples, v.len[i] / s.SS);
+    }
+    off[n] = s.total_bytes;
+    std::vector<uint8_t> flags(v.cont);
+    flags.insert(flags.end(), v.last.begin(), v.last.end());
+    CU(cudaMemcpyAsync(ctx->d_sp_view.p, view.data(), view.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(ctx->d_sp_flags.p, flags.data(), flags.size(), cudaMemcpyHostToDevice, st));
+    auto const *d_view = (unsigned long long const *)ctx->d_sp_view.p;
+    DetectParams q = dp;
+    q.offsets = d_view;
+    q.lengths = d_view + n + 1;
+    q.am_offsets = d_view + 2 * n + 1;
+    q.base = d_view + 3 * n + 2;
+    q.cont = (unsigned char const *)ctx->d_sp_flags.p;
+    q.last = q.cont + n;
+    q.n_streams = q.stream_end = (unsigned)n;
+    q.state = state;
+    q.train_scratch = train;
+    q.fm_out = nullptr;
+    CU(cudaEventRecord(ctx->ev_t[0], st));
+    launch_detect(ctx, q, sh, st, ctx->ev_t[1]);
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(&cnt, ctx->d_counters.p, sizeof(cnt), cudaMemcpyDeviceToHost, st));
+    CU(cudaEventRecord(ctx->ev_t[2], st));
+    CU(cudaEventSynchronize(ctx->ev_t[2]));
+    float a = 0, d = 0;
+    cudaEventElapsedTime(&a, ctx->ev_t[0], ctx->ev_t[1]);
+    cudaEventElapsedTime(&d, ctx->ev_t[1], ctx->ev_t[2]);
+    front_ms += a;
+    detect_ms += d;
+    return R433B_OK;
+}
+
+// k_split_compare over the listed segments; eq[k] = its seed equals its predecessor's end state
+int split_compare(r433b_ctx *ctx, std::vector<uint32_t> const &segs, std::vector<uint8_t> &eq)
+{
+    cudaStream_t const st = 0;
+    unsigned const m = (unsigned)segs.size();
+    if (!m) return R433B_OK;
+    size_t const n = eq.size();
+    unsigned *list = (unsigned *)ctx->d_sp_list.p;
+    std::vector<uint8_t> got(m);
+    CU(cudaMemcpyAsync(list, segs.data(), m * sizeof(unsigned), cudaMemcpyHostToDevice, st));
+    R4_LAUNCH(k_split_compare, (m + kSplitWarps - 1) / kSplitWarps, kSplitWarps * 32, 0, st,
+              (StreamState const *)ctx->d_sp_seed.p, (int const *)ctx->d_sp_seed_train.p, (StreamState const *)ctx->d_sp_state.p,
+              (int const *)ctx->d_sp_train.p, (unsigned const *)list, m, (unsigned char *)ctx->d_sp_eq.p, list + n);
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(got.data(), ctx->d_sp_eq.p, m, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    for (unsigned i = 0; i < m; ++i) eq[segs[i]] = got[i];
+    return R433B_OK;
+}
+
+// The split schedule on stream 0: copy-in, pass 0 (warm-ups -> seeds), pass 1 (every segment), rounds of rewalks until
+// every segment has started from its predecessor's exact end state, the merge, then the slicers over the merged packages.
+// An arena overflow in any launch grows the caps from what the device counted and runs the schedule again from pass 0.
+int run_split(r433b_ctx *ctx, r433b_batch const *b, Shape const &s, SplitPlan const &p, DetectParams const &dp0,
+        DetectCounters &cnt)
+{
+    cudaStream_t const st = 0;
+    size_t const n = p.stream.size(), ns = b->n_streams, tr = (size_t)kTrainInts * sizeof(int);
+    uint64_t const bb = s.settings.block_bytes;
+    for (auto [buf, bytes] : {std::pair<DevBuf *, size_t>{&ctx->d_sp_state, n * sizeof(StreamState)}, {&ctx->d_sp_train, n * tr},
+                              {&ctx->d_sp_seed, n * sizeof(StreamState)}, {&ctx->d_sp_seed_train, n * tr},
+                              {&ctx->d_sp_rw_state, ns * sizeof(StreamState)}, {&ctx->d_sp_rw_train, ns * tr},
+                              {&ctx->d_log, n * kLogCap * 2 * sizeof(unsigned)}, {&ctx->d_sp_view, (4 * n + 2) * sizeof(uint64_t)},
+                              {&ctx->d_sp_flags, 2 * n}, {&ctx->d_sp_list, (3 * n + 2) * sizeof(unsigned)}, {&ctx->d_sp_eq, n}})
+        if (int r = dev_reserve(ctx, *buf, bytes)) return r;
+    StreamState *const state = (StreamState *)ctx->d_sp_state.p, *const rw_state = (StreamState *)ctx->d_sp_rw_state.p;
+    int *const train = (int *)ctx->d_sp_train.p, *const rw_train = (int *)ctx->d_sp_rw_train.p;
+    unsigned *const list = (unsigned *)ctx->d_sp_list.p, *const start_seq = list + n, *const pkg_base = start_seq + n;
+    DetectParams dp = dp0;
+    dp.log_scratch = (unsigned *)ctx->d_log.p;
+
+    CU(cudaEventRecord(ctx->ev[0], st));
+    if (int r = copy_in(ctx, b, s, st)) return r;
+    CU(cudaEventRecord(ctx->ev[1], st));
+
+    // pass 0 walks the warm-up in front of every segment but a stream's first (those slots walk nothing), pass 1 the
+    // segments; slot k is segment k in both
+    SplitLaunch warm, walk;
+    std::vector<uint32_t> later; // every segment but a stream's first
+    for (size_t k = 0; k < n; ++k) {
+        bool const first = p.first[k] == k, last = k + 1 == n || p.first[k + 1] != p.first[k];
+        uint64_t const o = ctx->offsets[p.stream[k]], w0 = first || p.begin[k] < p.warmup * bb ? 0 : p.begin[k] - p.warmup * bb;
+        warm.add(o + w0, first ? 0 : p.begin[k] - w0, w0 / s.SS, false, false);
+        walk.add(o + p.begin[k], p.bytes[k], p.begin[k] / s.SS, !first, last);
+        if (!first) later.push_back((uint32_t)k);
+    }
+    float front_ms = 0, detect_ms = 0;
+    unsigned launches = 0, rewalks = 0, rounds = 0;
+    DetectCounters warm_cnt{};
+    std::vector<uint32_t> final_walk, launch_lo, map_off, seg_of;
+    for (int attempt = 0;; ++attempt) {
+        if (int r = bind_detector_arenas(ctx, dp)) return r;
+        CU(cudaMemsetAsync(ctx->d_counters.p, 0, 64, st));
+        if (int r = split_launch(ctx, dp, s, warm, state, train, warm_cnt, front_ms, detect_ms)) return r;
+        launches++;
+        // the warm-ups' packages are not kept: the arenas start again behind them
+        CU(cudaMemsetAsync(ctx->d_counters.p, 0, 64, st));
+        CU(cudaMemcpyAsync(ctx->d_sp_seed.p, state, n * sizeof(StreamState), cudaMemcpyDeviceToDevice, st));
+        CU(cudaMemcpyAsync(ctx->d_sp_seed_train.p, train, n * tr, cudaMemcpyDeviceToDevice, st));
+        CU(cudaMemsetAsync(start_seq, 0, n * sizeof(unsigned), st));
+        if (ctx->spoil_seed) { // only the copy that is compared: pass 1 starts from the seeds as they were
+            R4_LAUNCH(k_split_spoil, (unsigned)((n + 127) / 128), 128, 0, st, (StreamState *)ctx->d_sp_seed.p,
+                      (int *)ctx->d_sp_seed_train.p, (unsigned)n);
+            CU(cudaGetLastError());
+        }
+        if (int r = split_launch(ctx, dp, s, walk, state, train, cnt, front_ms, detect_ms)) return r;
+        launches++;
+        final_walk.assign(n, 0);
+        launch_lo = {0, cnt.pkgs};
+        map_off = {0};
+        seg_of.resize(n);
+        for (size_t k = 0; k < n; ++k) seg_of[k] = (uint32_t)k;
+        rewalks = rounds = 0;
+        // rounds: every stream's first segment whose seed was rejected is walked again from its predecessor's end state
+        std::vector<uint8_t> eq(n, 1);
+        if (!cnt.overflow)
+            if (int r = split_compare(ctx, later, eq)) return r;
+        auto frontier = [&](size_t k, std::vector<uint32_t> &out) { // the first rejected segment from k on, in k's stream
+            for (; k < n && p.first[k] == p.first[k - 1]; ++k)
+                if (!eq[k]) {
+                    out.push_back((uint32_t)k);
+                    return;
+                }
+        };
+        std::vector<uint32_t> rw, next, succ;
+        for (size_t k = 0; k < n; ++k)
+            if (p.first[k] == k && k + 1 < n) frontier(k + 1, rw);
+        while (!rw.empty() && !cnt.overflow) {
+            unsigned const m = (unsigned)rw.size(), grid = (m + kSplitWarps - 1) / kSplitWarps;
+            rounds++;
+            rewalks += m;
+            CU(cudaMemcpyAsync(list, rw.data(), m * sizeof(unsigned), cudaMemcpyHostToDevice, st));
+            R4_LAUNCH(k_split_gather, grid, kSplitWarps * 32, 0, st, (StreamState const *)state, (int const *)train,
+                      (unsigned const *)list, m, rw_state, rw_train, start_seq);
+            CU(cudaGetLastError());
+            SplitLaunch again;
+            for (uint32_t k : rw) again.add(walk.off[k], walk.len[k], walk.base[k], true, walk.last[k] != 0);
+            if (int r = split_launch(ctx, dp, s, again, rw_state, rw_train, cnt, front_ms, detect_ms)) return r;
+            launches++;
+            R4_LAUNCH(k_split_scatter, grid, kSplitWarps * 32, 0, st, (StreamState const *)rw_state, (int const *)rw_train,
+                      (unsigned const *)list, m, state, train);
+            CU(cudaGetLastError());
+            map_off.push_back((uint32_t)seg_of.size());
+            seg_of.insert(seg_of.end(), rw.begin(), rw.end());
+            launch_lo.push_back(cnt.pkgs);
+            succ.clear();
+            for (uint32_t k : rw) {
+                final_walk[k] = rounds;
+                if (k + 1 < n && p.first[k + 1] == p.first[k]) succ.push_back(k + 1);
+            }
+            if (int r = split_compare(ctx, succ, eq)) return r;
+            next.clear();
+            for (uint32_t k : succ) frontier(k, next);
+            rw.swap(next);
+        }
+        if (!cnt.overflow) break;
+        // an arena was too small: the counters hold what the launches so far needed, the launches still to come more
+        ctx->pkg_cap = std::max<size_t>(ctx->pkg_cap, (size_t)cnt.pkgs * 2 + 64);
+        ctx->pool_cap = std::max<size_t>(ctx->pool_cap, (size_t)cnt.pool * 2 + 4096);
+        if (attempt == 2) return fail(ctx, R433B_EOVERFLOW, "package arena overflow");
+    }
+
+    // the merge: the packages of every segment's last walk, renumbered, into a second set of arenas that then swaps in
+    size_t const n_launch = launch_lo.size() - 1, n_src = launch_lo.back();
+    std::vector<uint32_t> tab;
+    tab.reserve(3 * n + 2 * n_launch + 1 + seg_of.size() + 1);
+    tab.insert(tab.end(), p.stream.begin(), p.stream.end());
+    tab.insert(tab.end(), p.first.begin(), p.first.end());
+    tab.insert(tab.end(), final_walk.begin(), final_walk.end());
+    tab.insert(tab.end(), launch_lo.begin(), launch_lo.end());
+    tab.insert(tab.end(), map_off.begin(), map_off.end());
+    tab.insert(tab.end(), seg_of.begin(), seg_of.end());
+    tab.push_back(0); // the pool cursor
+    if (int r = dev_reserve(ctx, ctx->d_sp_tab, tab.size() * sizeof(uint32_t))) return r;
+    if (int r = dev_reserve(ctx, ctx->d_sp_pkgs, ctx->pkg_cap * sizeof(r433b_package))) return r;
+    if (int r = dev_reserve(ctx, ctx->d_sp_ppool, ctx->pool_cap * sizeof(int))) return r;
+    if (int r = dev_reserve(ctx, ctx->d_sp_gpool, ctx->pool_cap * sizeof(int))) return r;
+    CU(cudaMemcpyAsync(ctx->d_sp_tab.p, tab.data(), tab.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+    unsigned const *t = (unsigned const *)ctx->d_sp_tab.p;
+    SplitMerge mg{};
+    mg.n_segs = (unsigned)n;
+    mg.n_launches = (unsigned)n_launch;
+    mg.seg_stream = t;
+    mg.seg_first = t + n;
+    mg.final_walk = t + 2 * n;
+    mg.launch_lo = t + 3 * n;
+    mg.map_off = mg.launch_lo + n_launch + 1;
+    mg.seg_of = mg.map_off + n_launch;
+    mg.pool_cursor = (unsigned *)ctx->d_sp_tab.p + tab.size() - 1;
+    mg.start_seq = start_seq;
+    mg.state = state;
+    mg.pkg_base = pkg_base;
+    mg.src = (r433b_package const *)ctx->d_pkgs.p;
+    mg.src_pulse = (int const *)ctx->d_ppool.p;
+    mg.src_gap = (int const *)ctx->d_gpool.p;
+    mg.dst = (r433b_package *)ctx->d_sp_pkgs.p;
+    mg.dst_pulse = (int *)ctx->d_sp_ppool.p;
+    mg.dst_gap = (int *)ctx->d_sp_gpool.p;
+    CU(cudaEventRecord(ctx->ev_t[3], st));
+    R4_LAUNCH(k_split_merge_scan, 1, 32, 0, st, mg);
+    if (n_src) R4_LAUNCH(k_split_merge, (unsigned)((n_src + kSplitWarps - 1) / kSplitWarps), kSplitWarps * 32, 0, st, mg);
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(ctx->ev_t[4], st));
+    unsigned kept[2] = {0, 0}; // packages, pool entries
+    CU(cudaMemcpyAsync(&kept[0], pkg_base + n, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(&kept[1], mg.pool_cursor, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    std::swap(ctx->d_pkgs, ctx->d_sp_pkgs);
+    std::swap(ctx->d_ppool, ctx->d_sp_ppool);
+    std::swap(ctx->d_gpool, ctx->d_sp_gpool);
+    if (int r = check_pair_index(ctx, kept[0])) return r;
+    ctx->n_pkgs = kept[0];
+    ctx->pool_used = kept[1];
+    GroupRange all{};
+    all.pkg_end = ctx->n_pkgs;
+    if (int r = slice_ranges(ctx, std::vector<GroupRange>{all}, ctx->n_pkgs, ctx->pool_used, st)) return r;
+
+    // the pass-0 shortcuts count too
+    cnt.front_redone += warm_cnt.front_redone;
+    cnt.front_repairs += warm_cnt.front_repairs;
+    cnt.idle_skipped += warm_cnt.idle_skipped;
+    cnt.idle_rewalks += warm_cnt.idle_rewalks;
+    cnt.chain_folds += warm_cnt.chain_folds;
+    cnt.chain_fm_rebuilds += warm_cnt.chain_fm_rebuilds;
+    cudaEventElapsedTime(&ctx->timing.h2d_ms, ctx->ev[0], ctx->ev[1]);
+    cudaEventElapsedTime(&ctx->timing.split_merge_ms, ctx->ev_t[3], ctx->ev_t[4]);
+    cudaEventElapsedTime(&ctx->timing.total_ms, ctx->ev[0], ctx->ev[3]);
+    ctx->timing.front_ms = front_ms;
+    ctx->timing.detect_ms = detect_ms;
+    ctx->timing.detect_launches = launches;
+    ctx->timing.split_segments = (uint32_t)n;
+    ctx->timing.split_rewalks = rewalks;
+    ctx->timing.split_rounds = rounds;
+    return R433B_OK;
+}
+
 // rtl_433 -r on every stream of the batch; with a chain, stream i is the next chunk of slot i's file (r433b.h)
 int process_iq(r433b_ctx *ctx, r433b_batch const *b, r433b_chain *ch, uint8_t const *last)
 {
@@ -1015,12 +1355,19 @@ int process_iq(r433b_ctx *ctx, r433b_batch const *b, r433b_chain *ch, uint8_t co
     ctx->pkg_cap = std::max<size_t>(ctx->pkg_cap, ctx->min_caps[0] ? ctx->min_caps[0] : (size_t)b->n_streams * 16 + 1024);
     ctx->pool_cap = std::max<size_t>(ctx->pool_cap, ctx->min_caps[1] ? ctx->min_caps[1] : ctx->pkg_cap * 128);
     ctx->arena_cap = std::max<size_t>(ctx->arena_cap, ctx->min_caps[2] ? ctx->min_caps[2] : s.total_bytes / 2 + (1u << 20));
-    uint64_t slice_samples;
-    int const G = time_slices(ctx, b, s, slice_samples);
+    ctx->timing.split_segments = ctx->timing.split_rewalks = ctx->timing.split_rounds = 0;
+    ctx->timing.split_merge_ms = 0;
     DetectCounters cnt{};
     int r = kFellBack;
-    if (G > 1) r = run_time_sliced(ctx, b, s, G, slice_samples, dp, cnt);
-    if (r == kFellBack) r = run_sequential(ctx, b, s, dp, ch, G > 1, cnt);
+    SplitPlan plan;
+    if (!ch && plan_split(ctx, b, s, plan)) {
+        r = run_split(ctx, b, s, plan, dp, cnt);
+    } else {
+        uint64_t slice_samples;
+        int const G = time_slices(ctx, b, s, slice_samples);
+        if (G > 1) r = run_time_sliced(ctx, b, s, G, slice_samples, dp, cnt);
+        if (r == kFellBack) r = run_sequential(ctx, b, s, dp, ch, G > 1, cnt);
+    }
     if (r) return r;
     ctx->timing.front_redone = cnt.front_redone;
     ctx->timing.front_repairs = cnt.front_repairs;

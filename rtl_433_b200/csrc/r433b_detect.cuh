@@ -47,6 +47,10 @@ namespace r433b {
 constexpr int kTrainInts = 4 * kMaxPulses; // per-stream scratch: ook pulse/gap, fsk pulse/gap
 constexpr int kDetectWarps = 4;            // warps (streams) per CTA
 constexpr int kDetectCtasPerSm = 8;        // 32 warps per SM (64 registers): 4096 streams are co-resident on 132 SMs
+// R433B_SPLIT_AUTO (r433b_set_split): a batch of fewer streams than resident k_detect warps splits the streams of at least
+// kSplitMinSegments segments of at least kSplitMinSegmentBlocks blocks, the segments sized for about one slot per warp
+constexpr int kSplitMinSegments = 4;
+constexpr int kSplitMinSegmentBlocks = 2;
 
 constexpr int kAmStride = kChunk / 2 + 1;  // words between lane chunks of the 16-bit AM tile (odd: conflict-free)
 constexpr int kAmWords = 32 * kAmStride;

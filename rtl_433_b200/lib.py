@@ -33,7 +33,7 @@ EXPORTS = ["r433b_create", "r433b_destroy", "r433b_last_error", "r433b_set_level
            "r433b_dispatch_r_devices_parallel", "r433b_analyze", "r433b_analysis_get", "r433b_analysis_text",
            "r433b_analysis_events", "r433b_submit", "r433b_wait", "r433b_grab_plan", "r433b_grab_copy", "r433b_grab_tail",
            "r433b_chain_create", "r433b_chain_destroy", "r433b_process_chained", "r433b_chain_base",
-           "r433b_chain_grab"]
+           "r433b_chain_grab", "r433b_set_split"]
 
 
 def build(force=False, verbose=False):
@@ -114,8 +114,11 @@ class Timing(C.Structure):
                 ("front_ms", C.c_float), ("front_launches", C.c_uint32), ("front_redone", C.c_uint32),
                 ("front_repairs", C.c_uint32), ("idle_skipped", C.c_uint32), ("idle_rewalks", C.c_uint32),
                 ("grab_ms", C.c_float), ("chain_folds", C.c_uint32), ("chain_fm_rebuilds", C.c_uint32),
-                ("grab_ring_ms", C.c_float)]
+                ("grab_ring_ms", C.c_float), ("split_segments", C.c_uint32), ("split_rewalks", C.c_uint32),
+                ("split_rounds", C.c_uint32), ("split_merge_ms", C.c_float)]
 
+
+SPLIT_AUTO = 0xFFFFFFFF  # r433b_set_split: segment size chosen from the batch's shape
 
 GRAB_ALL, GRAB_UNKNOWN, GRAB_KNOWN, GRAB_UNDECODED = 1, 2, 3, 4
 GRAB_RING = 12 * 262144  # SIGNAL_GRABBER_BUFFER
@@ -165,6 +168,7 @@ def load():
     L.r433b_set_levels.argtypes = [C.c_void_p, C.c_int, C.c_float, C.c_float, C.c_float]
     L.r433b_set_fm_low_pass.argtypes = [C.c_void_p, C.c_float]
     L.r433b_set_pipeline.argtypes = [C.c_void_p, C.c_int]
+    L.r433b_set_split.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32]
     L.r433b_set_devices.argtypes = [C.c_void_p, C.POINTER(Device), C.c_uint32]
     L.r433b_set_r_devices.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
     L.r433b_process.argtypes = [C.c_void_p, C.POINTER(Batch)]
@@ -411,6 +415,11 @@ class Context:
 
     def set_pipeline(self, groups):
         self._check(self.L.r433b_set_pipeline(self.h, groups))
+
+    def set_split(self, segment_blocks, warmup_blocks=1):
+        """Segmented replay of long streams (include/r433b.h: r433b_set_split): segment_blocks 0 = off, SPLIT_AUTO =
+        chosen from the batch.  Results are those of the unsplit batch."""
+        self._check(self.L.r433b_set_split(self.h, segment_blocks, warmup_blocks))
 
     def set_devices(self, devs):
         arr = (Device * len(devs))()
