@@ -165,7 +165,8 @@ int r433b_set_pipeline(r433b_ctx *ctx, int groups);
      resident warp.
    - warmup_blocks is 1 .. segment_blocks (R433B_EINVAL otherwise; with R433B_SPLIT_AUTO it is capped to the chosen
      segment).  A warm-up never reaches in front of its stream's start.
-   - Batches with want_stages, chained batches and batches in which no stream has two segments run unsplit.
+   - Batches with want_stages, chained batches (unless their chain opted in, see r433b_chain_split) and batches in
+     which no stream has two segments run unsplit.
    - Memory on the device, per slot: the state and pulse trains of the walk and of its seed (about 40 KB), plus one
      rewalk slot per stream.  r433b_timing.split_* report what the schedule did. */
 #define R433B_SPLIT_AUTO 0xffffffffu
@@ -220,7 +221,9 @@ int r433b_process(r433b_ctx *ctx, r433b_batch const *batch);
    - A chain belongs to the context that created it and owns its device memory: per slot the carried state, the
      pulse-train scratch (19.2 KB) and a copy of both (a batch whose result arenas overflow runs again from it), about
      40 KB per slot.  r433b_destroy() frees the device memory of the context's chains; such a chain only accepts
-     r433b_chain_destroy().  After a failed r433b_process_chained() the chain is undefined. */
+     r433b_chain_destroy().  After a failed r433b_process_chained() the chain is undefined.
+   - A chained batch walks each slot's chunk on one warp, whatever r433b_set_split says; r433b_chain_split below lets
+     one chain's batches split each chunk across warps instead. */
 typedef struct r433b_chain r433b_chain;
 /* every slot at a file start */
 int r433b_chain_create(r433b_ctx *ctx, uint32_t n_streams, r433b_chain **out);
@@ -253,6 +256,17 @@ int r433b_chain_base(r433b_chain const *chain, uint32_t stream, uint64_t *first_
      lost.  When appending a batch to the rings fails, the call fails and the chain's rings no longer match its runs:
      later chained batches and plans of that chain return R433B_ESTATE. */
 int r433b_chain_grab(r433b_chain *chain, int mode);
+/* Segmented replay for the chained batches of this chain: stream i's chunk is cut into segments of segment_blocks
+   blocks (R433B_SPLIT_AUTO: chosen from the batch as r433b_set_split does), segment 0 starts from the state the chain
+   carried for slot i, the others from warm-up seeds, verified and rewalked as in r433b_set_split.  Results equal the
+   unsplit chain's, so it may be turned on, off (0) or changed between any two chained batches.
+   - warmup_blocks is 1 .. segment_blocks (R433B_EINVAL otherwise, and for a chain whose context is gone).  Warm-ups
+     lie inside the chunk: a segment near the chunk start is seeded from the chunk start, and verified like any other.
+   - Batches with want_stages, and batches in which no chunk has two segments, run unsplit.  r433b_timing.split_*
+     report what the schedule did.  The chain's state is written once the whole batch has succeeded, so an arena
+     overflow reruns the schedule from the state the chain carried.
+   - Memory on the device: that of r433b_set_split for the batch's segments, in the context. */
+int r433b_chain_split(r433b_chain *chain, uint32_t segment_blocks, uint32_t warmup_blocks);
 
 /* Copy the compact results to host memory owned by the context. */
 int r433b_fetch(r433b_ctx *ctx, r433b_results *out);

@@ -176,6 +176,8 @@ struct r433b_chain {
     std::vector<uint64_t> next;    // ... whose next chunk starts at this absolute sample
     std::vector<uint64_t> base;    // first sample of slot i's chunk in the last chained batch
     ChainSettings settings{};
+    // segmented replay of this chain's batches (r433b_chain_split): segment / warm-up blocks, 0: off
+    uint32_t split_blocks = 0, split_warmup = 1;
     // signal grabber (r433b_chain_grab): each slot is its own run with a kGrabRingBytes ring on the device
     int grab_mode = 0;
     bool grab_pending = false;     // the last chained batch has not been planned yet
@@ -386,6 +388,16 @@ int r433b_set_split(r433b_ctx *ctx, uint32_t segment_blocks, uint32_t warmup_blo
         return fail(ctx, R433B_EINVAL, "r433b_set_split: warmup_blocks must be 1 .. segment_blocks");
     ctx->split_blocks = segment_blocks;
     ctx->split_warmup = segment_blocks ? warmup_blocks : 1;
+    return R433B_OK;
+}
+
+int r433b_chain_split(r433b_chain *chain, uint32_t segment_blocks, uint32_t warmup_blocks)
+{
+    if (!chain || !chain->ctx) return R433B_EINVAL;
+    if (segment_blocks && (warmup_blocks < 1 || (segment_blocks != R433B_SPLIT_AUTO && warmup_blocks > segment_blocks)))
+        return fail(chain->ctx, R433B_EINVAL, "r433b_chain_split: warmup_blocks must be 1 .. segment_blocks");
+    chain->split_blocks = segment_blocks;
+    chain->split_warmup = segment_blocks ? warmup_blocks : 1;
     return R433B_OK;
 }
 
@@ -1037,13 +1049,16 @@ struct SplitPlan {
     uint64_t warmup = 1;                 // blocks
 };
 
-// false: the batch runs unsplit (splitting off, stage arrays, or no stream of two segments)
-bool plan_split(r433b_ctx const *ctx, r433b_batch const *b, Shape const &s, SplitPlan &p)
+// Segments of segment_blocks blocks (R433B_SPLIT_AUTO: chosen from the batch) behind warm-ups of warmup_blocks, cut from
+// each stream's used bytes (a chained batch's: each slot's chunk).  false: the batch runs unsplit (splitting off, stage
+// arrays, or no stream of two segments).
+bool plan_split(r433b_ctx const *ctx, r433b_batch const *b, Shape const &s, uint32_t segment_blocks, uint32_t warmup_blocks,
+        SplitPlan &p)
 {
-    if (!ctx->split_blocks || b->want_stages || !b->n_streams) return false;
+    if (!segment_blocks || b->want_stages || !b->n_streams) return false;
     uint64_t const bb = s.settings.block_bytes;
-    uint64_t seg = ctx->split_blocks, min_blocks = 0;
-    if (ctx->split_blocks == R433B_SPLIT_AUTO) {
+    uint64_t seg = segment_blocks, min_blocks = 0;
+    if (segment_blocks == R433B_SPLIT_AUTO) {
         uint64_t const warps = (uint64_t)ctx->n_sms * kDetectCtasPerSm * kDetectWarps, n = b->n_streams;
         if (n >= warps) return false;
         uint64_t blocks = 0;
@@ -1051,7 +1066,7 @@ bool plan_split(r433b_ctx const *ctx, r433b_batch const *b, Shape const &s, Spli
         seg = std::max<uint64_t>(kSplitMinSegmentBlocks, (blocks + warps - 1) / warps);
         min_blocks = seg * kSplitMinSegments;
     }
-    p.warmup = std::min<uint64_t>(ctx->split_warmup, seg);
+    p.warmup = std::min<uint64_t>(warmup_blocks, seg);
     bool any = false;
     for (uint32_t i = 0; i < b->n_streams; ++i) {
         uint64_t const len = ctx->lengths[i], blocks = (len + bb - 1) / bb;
@@ -1157,8 +1172,11 @@ int split_compare(r433b_ctx *ctx, std::vector<uint32_t> const &segs, std::vector
 // The split schedule on stream 0: copy-in, pass 0 (warm-ups -> seeds), pass 1 (every segment), rounds of rewalks until
 // every segment has started from its predecessor's exact end state, the merge, then the slicers over the merged packages.
 // An arena overflow in any launch grows the caps from what the device counted and runs the schedule again from pass 0.
+// With a chain, stream i's segments lie at the chain's base for slot i, the first starts from the state the chain
+// carried (loaded in front of pass 1, so a rerun loads it again), the last ends as the chunk does (last[i]), and the
+// chain takes the last's end state once everything has succeeded.
 int run_split(r433b_ctx *ctx, r433b_batch const *b, Shape const &s, SplitPlan const &p, DetectParams const &dp0,
-        DetectCounters &cnt)
+        r433b_chain *ch, uint8_t const *last_chunk, DetectCounters &cnt)
 {
     cudaStream_t const st = 0;
     size_t const n = p.stream.size(), ns = b->n_streams, tr = (size_t)kTrainInts * sizeof(int);
@@ -1167,11 +1185,13 @@ int run_split(r433b_ctx *ctx, r433b_batch const *b, Shape const &s, SplitPlan co
                               {&ctx->d_sp_seed, n * sizeof(StreamState)}, {&ctx->d_sp_seed_train, n * tr},
                               {&ctx->d_sp_rw_state, ns * sizeof(StreamState)}, {&ctx->d_sp_rw_train, ns * tr},
                               {&ctx->d_log, n * kLogCap * 2 * sizeof(unsigned)}, {&ctx->d_sp_view, (4 * n + 2) * sizeof(uint64_t)},
-                              {&ctx->d_sp_flags, 2 * n}, {&ctx->d_sp_list, (3 * n + 2) * sizeof(unsigned)}, {&ctx->d_sp_eq, n}})
+                              {&ctx->d_sp_flags, 2 * n}, {&ctx->d_sp_list, (3 * n + 2 + 2 * ns) * sizeof(unsigned)},
+                              {&ctx->d_sp_eq, n}})
         if (int r = dev_reserve(ctx, *buf, bytes)) return r;
     StreamState *const state = (StreamState *)ctx->d_sp_state.p, *const rw_state = (StreamState *)ctx->d_sp_rw_state.p;
     int *const train = (int *)ctx->d_sp_train.p, *const rw_train = (int *)ctx->d_sp_rw_train.p;
     unsigned *const list = (unsigned *)ctx->d_sp_list.p, *const start_seq = list + n, *const pkg_base = start_seq + n;
+    unsigned *const slot_first = pkg_base + n + 2, *const slot_last = slot_first + ns; // per stream: its first / last segment
     DetectParams dp = dp0;
     dp.log_scratch = (unsigned *)ctx->d_log.p;
 
@@ -1182,14 +1202,20 @@ int run_split(r433b_ctx *ctx, r433b_batch const *b, Shape const &s, SplitPlan co
     // pass 0 walks the warm-up in front of every segment but a stream's first (those slots walk nothing), pass 1 the
     // segments; slot k is segment k in both
     SplitLaunch warm, walk;
-    std::vector<uint32_t> later; // every segment but a stream's first
+    std::vector<uint32_t> later, slots(2 * ns); // every segment but a stream's first; each stream's first and last
     for (size_t k = 0; k < n; ++k) {
+        uint32_t const i = p.stream[k];
         bool const first = p.first[k] == k, last = k + 1 == n || p.first[k + 1] != p.first[k];
-        uint64_t const o = ctx->offsets[p.stream[k]], w0 = first || p.begin[k] < p.warmup * bb ? 0 : p.begin[k] - p.warmup * bb;
-        warm.add(o + w0, first ? 0 : p.begin[k] - w0, w0 / s.SS, false, false);
-        walk.add(o + p.begin[k], p.bytes[k], p.begin[k] / s.SS, !first, last);
+        uint64_t const o = ctx->offsets[i], w0 = first || p.begin[k] < p.warmup * bb ? 0 : p.begin[k] - p.warmup * bb;
+        uint64_t const base = ch ? ctx->chain_base[i] : 0;
+        warm.add(o + w0, first ? 0 : p.begin[k] - w0, base + w0 / s.SS, false, false);
+        walk.add(o + p.begin[k], p.bytes[k], base + p.begin[k] / s.SS, first ? ch && ch->open[i] : true,
+                 last && (!ch || last_chunk[i]));
         if (!first) later.push_back((uint32_t)k);
+        if (first) slots[i] = (uint32_t)k;
+        if (last) slots[ns + i] = (uint32_t)k;
     }
+    if (ch) CU(cudaMemcpyAsync(slot_first, slots.data(), 2 * ns * sizeof(unsigned), cudaMemcpyHostToDevice, st));
     float front_ms = 0, detect_ms = 0;
     unsigned launches = 0, rewalks = 0, rounds = 0;
     DetectCounters warm_cnt{};
@@ -1204,6 +1230,12 @@ int run_split(r433b_ctx *ctx, r433b_batch const *b, Shape const &s, SplitPlan co
         CU(cudaMemcpyAsync(ctx->d_sp_seed.p, state, n * sizeof(StreamState), cudaMemcpyDeviceToDevice, st));
         CU(cudaMemcpyAsync(ctx->d_sp_seed_train.p, train, n * tr, cudaMemcpyDeviceToDevice, st));
         CU(cudaMemsetAsync(start_seq, 0, n * sizeof(unsigned), st));
+        if (ch) {
+            R4_LAUNCH(k_split_chain_in, (unsigned)((ns + kSplitWarps - 1) / kSplitWarps), kSplitWarps * 32, 0, st,
+                      (StreamState const *)ch->d_state.p, (int const *)ch->d_train.p, (unsigned char const *)ch->d_flags.p,
+                      (unsigned const *)slot_first, (unsigned)ns, state, train, start_seq);
+            CU(cudaGetLastError());
+        }
         if (ctx->spoil_seed) { // only the copy that is compared: pass 1 starts from the seeds as they were
             R4_LAUNCH(k_split_spoil, (unsigned)((n + 127) / 128), 128, 0, st, (StreamState *)ctx->d_sp_seed.p,
                       (int *)ctx->d_sp_seed_train.p, (unsigned)n);
@@ -1320,6 +1352,13 @@ int run_split(r433b_ctx *ctx, r433b_batch const *b, Shape const &s, SplitPlan co
     GroupRange all{};
     all.pkg_end = ctx->n_pkgs;
     if (int r = slice_ranges(ctx, std::vector<GroupRange>{all}, ctx->n_pkgs, ctx->pool_used, st)) return r;
+    if (ch) {
+        R4_LAUNCH(k_split_chain_out, (unsigned)((ns + kSplitWarps - 1) / kSplitWarps), kSplitWarps * 32, 0, st,
+                  (StreamState const *)state, (int const *)train, (unsigned const *)slot_first, (unsigned const *)slot_last,
+                  (unsigned const *)start_seq, (unsigned const *)pkg_base, (unsigned)ns, (StreamState *)ch->d_state.p,
+                  (int *)ch->d_train.p);
+        CU(cudaGetLastError());
+    }
 
     // the pass-0 shortcuts count too
     cnt.front_redone += warm_cnt.front_redone;
@@ -1360,8 +1399,10 @@ int process_iq(r433b_ctx *ctx, r433b_batch const *b, r433b_chain *ch, uint8_t co
     DetectCounters cnt{};
     int r = kFellBack;
     SplitPlan plan;
-    if (!ch && plan_split(ctx, b, s, plan)) {
-        r = run_split(ctx, b, s, plan, dp, cnt);
+    // a chain splits only when it opted in (r433b_chain_split): the context's setting is for unchained batches
+    uint32_t const split_blocks = ch ? ch->split_blocks : ctx->split_blocks, split_warmup = ch ? ch->split_warmup : ctx->split_warmup;
+    if (plan_split(ctx, b, s, split_blocks, split_warmup, plan)) {
+        r = run_split(ctx, b, s, plan, dp, ch, last, cnt);
     } else {
         uint64_t slice_samples;
         int const G = time_slices(ctx, b, s, slice_samples);

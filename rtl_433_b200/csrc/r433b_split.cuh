@@ -1,7 +1,7 @@
 // r433b_split.cuh -- segmented replay (DESIGN §7c): the device side of the schedule that walks the segments of one long
 // stream on separate warps.  k_front / k_detect walk the segments as chained chunks; the kernels here compare a segment's
-// start state with its predecessor's end state, move start / end states between the slots and a rewalk launch, and
-// merge the packages of every segment's last walk into the batch's arenas.
+// start state with its predecessor's end state, move start / end states between the slots, a rewalk launch and the
+// slots of a chain, and merge the packages of every segment's last walk into the batch's arenas.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -102,6 +102,14 @@ __global__ void k_split_spoil(StreamState *seed, int *seed_train, unsigned n)
     }
 }
 
+// One warp: the pulse trains of one slot (kTrainInts ints, 16-byte aligned) into another, in int4 words
+__device__ __forceinline__ void split_copy_train(int const *src, int *dst, int lane)
+{
+    int4 const *s = reinterpret_cast<int4 const *>(src);
+    int4 *d = reinterpret_cast<int4 *>(dst);
+    for (int j = lane; j < kTrainInts / 4; j += 32) d[j] = s[j];
+}
+
 // One warp per listed segment k: the rewalk launch's stream i starts from the end state (and trains) of segment k - 1;
 // start_seq[k] is the seq it starts from
 __global__ void __launch_bounds__(kSplitWarps * 32) k_split_gather(StreamState const *state, int const *train,
@@ -111,9 +119,7 @@ __global__ void __launch_bounds__(kSplitWarps * 32) k_split_gather(StreamState c
     int const lane = threadIdx.x & 31;
     if (i >= n) return;
     unsigned const k = segs[i];
-    int4 const *src = reinterpret_cast<int4 const *>(train + (size_t)(k - 1) * kTrainInts);
-    int4 *dst = reinterpret_cast<int4 *>(rw_train + (size_t)i * kTrainInts);
-    for (int j = lane; j < kTrainInts / 4; j += 32) dst[j] = src[j];
+    split_copy_train(train + (size_t)(k - 1) * kTrainInts, rw_train + (size_t)i * kTrainInts, lane);
     if (lane == 0) {
         rw_state[i] = state[k - 1];
         start_seq[k] = state[k - 1].seq;
@@ -128,10 +134,45 @@ __global__ void __launch_bounds__(kSplitWarps * 32) k_split_scatter(StreamState 
     int const lane = threadIdx.x & 31;
     if (i >= n) return;
     unsigned const k = segs[i];
-    int4 const *src = reinterpret_cast<int4 const *>(rw_train + (size_t)i * kTrainInts);
-    int4 *dst = reinterpret_cast<int4 *>(train + (size_t)k * kTrainInts);
-    for (int j = lane; j < kTrainInts / 4; j += 32) dst[j] = src[j];
+    split_copy_train(rw_train + (size_t)i * kTrainInts, train + (size_t)k * kTrainInts, lane);
     if (lane == 0) state[k] = rw_state[i];
+}
+
+// Chained batches (r433b_chain_split), one warp per chain slot i whose file goes on (cont[i]): the slot's first segment
+// first[i] starts from the state and trains the chain carried, and from its seq.  A slot that starts a file keeps the
+// reset state pass 0 left in that segment's slot, and start_seq 0.
+__global__ void __launch_bounds__(kSplitWarps * 32) k_split_chain_in(StreamState const *chain_state,
+        int const *chain_train, unsigned char const *cont, unsigned const *first, unsigned n, StreamState *state,
+        int *train, unsigned *start_seq)
+{
+    unsigned const i = blockIdx.x * kSplitWarps + (threadIdx.x >> 5);
+    int const lane = threadIdx.x & 31;
+    if (i >= n || !cont[i]) return;
+    unsigned const k = first[i];
+    split_copy_train(chain_train + (size_t)i * kTrainInts, train + (size_t)k * kTrainInts, lane);
+    if (lane == 0) {
+        state[k] = chain_state[i];
+        start_seq[k] = chain_state[i].seq;
+    }
+}
+
+// After the merge, one warp per chain slot i: the chain goes on from the end state and trains of the slot's last
+// segment last[i].  That walk counted seq from its own start (a seed's counts the warm-up's packages), so the carried
+// seq is the slot's start seq plus the packages merged for the slot.
+__global__ void __launch_bounds__(kSplitWarps * 32) k_split_chain_out(StreamState const *state, int const *train,
+        unsigned const *first, unsigned const *last, unsigned const *start_seq, unsigned const *pkg_base, unsigned n,
+        StreamState *chain_state, int *chain_train)
+{
+    unsigned const i = blockIdx.x * kSplitWarps + (threadIdx.x >> 5);
+    int const lane = threadIdx.x & 31;
+    if (i >= n) return;
+    unsigned const k = last[i], f = first[i];
+    split_copy_train(train + (size_t)k * kTrainInts, chain_train + (size_t)i * kTrainInts, lane);
+    if (lane == 0) {
+        StreamState ss = state[k];
+        ss.seq = start_seq[f] + pkg_base[k + 1] - pkg_base[f];
+        chain_state[i] = ss;
+    }
 }
 
 // What the merge reads per segment and per walk (host-built, except start_seq and pkg_base)
@@ -173,7 +214,8 @@ __global__ void k_split_merge_scan(SplitMerge m)
 }
 
 // One warp per stored package: a package of its segment's last walk goes to pkg_base[seg] + (seq - start_seq) with the
-// batch's stream, the seq the one-warp walk gives it and its widths copied to the next free pool entries
+// batch's stream, the seq the one-warp walk gives it and its widths copied to the next free pool entries.  The seq goes
+// on from the stream's first segment's start seq: 0, or what a chained batch's slot carried.
 __global__ void __launch_bounds__(kSplitWarps * 32) k_split_merge(SplitMerge m)
 {
     unsigned const idx = blockIdx.x * kSplitWarps + (threadIdx.x >> 5);
@@ -198,7 +240,8 @@ __global__ void __launch_bounds__(kSplitWarps * 32) k_split_merge(SplitMerge m)
     }
     if (lane == 0) {
         k.stream = m.seg_stream[seg];
-        k.seq = m.pkg_base[seg] - m.pkg_base[m.seg_first[seg]] + rel;
+        unsigned const first = m.seg_first[seg];
+        k.seq = m.start_seq[first] + m.pkg_base[seg] - m.pkg_base[first] + rel;
         k.pulse_off = off;
         m.dst[m.pkg_base[seg] + rel] = k;
     }

@@ -33,7 +33,7 @@ EXPORTS = ["r433b_create", "r433b_destroy", "r433b_last_error", "r433b_set_level
            "r433b_dispatch_r_devices_parallel", "r433b_analyze", "r433b_analysis_get", "r433b_analysis_text",
            "r433b_analysis_events", "r433b_submit", "r433b_wait", "r433b_grab_plan", "r433b_grab_copy", "r433b_grab_tail",
            "r433b_chain_create", "r433b_chain_destroy", "r433b_process_chained", "r433b_chain_base",
-           "r433b_chain_grab", "r433b_set_split"]
+           "r433b_chain_grab", "r433b_set_split", "r433b_chain_split"]
 
 
 def build(force=False, verbose=False):
@@ -177,6 +177,7 @@ def load():
     L.r433b_process_chained.argtypes = [C.c_void_p, C.POINTER(Batch), C.c_void_p, C.c_void_p]
     L.r433b_chain_base.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint64)]
     L.r433b_chain_grab.argtypes = [C.c_void_p, C.c_int]
+    L.r433b_chain_split.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32]
     L.r433b_fetch.argtypes = [C.c_void_p, C.POINTER(Results)]
     L.r433b_get_timing.argtypes = [C.c_void_p, C.POINTER(Timing)]
     L.r433b_get_counts.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
@@ -379,6 +380,12 @@ class Chain:
         """Grab signals in `mode` (GRAB_*) on every slot, each its own run (include/r433b.h: r433b_chain_grab).  After
         each chained batch, ctx.grab_plan(mode) lists the grabs whose frames ended in it; ctx.grab_copy gathers them."""
         self.ctx._check(self.L.r433b_chain_grab(self.h, mode))
+
+    def split(self, segment_blocks, warmup_blocks=1):
+        """Segmented replay of this chain's batches (include/r433b.h: r433b_chain_split): each slot's chunk is walked in
+        segments of segment_blocks blocks, the first from the carried state; 0 = off, SPLIT_AUTO = chosen from the
+        batch.  Results are those of the unsplit chain; it may change between any two batches."""
+        self.ctx._check(self.L.r433b_chain_split(self.h, segment_blocks, warmup_blocks))
 
 
 class Context:
