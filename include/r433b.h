@@ -56,7 +56,7 @@ typedef struct r433b_device {
     uint32_t priority;
 } r433b_device;
 
-/* One batch of capture "files" (all of one format / rate / centre frequency).
+/* One batch of capture "files" (all of one format / rate / centre frequency; r433b_process_mixed takes them per stream).
    Stream i occupies bytes [offsets[i], offsets[i+1]) of `data`; offsets must be multiples
    of 16.  `data` is host memory (pageable or pinned) or, with data_on_device, device memory. */
 typedef struct r433b_batch {
@@ -133,6 +133,8 @@ typedef struct r433b_timing {
     uint32_t split_rewalks;  /* segments walked again from their predecessor's end state */
     uint32_t split_rounds;   /* rewalk launches */
     float split_merge_ms;    /* k_split_merge_scan + k_split_merge (device time) */
+    uint32_t mixed_classes;  /* r433b_process_mixed: detector classes of the batch (0 for every other batch) */
+    float mixed_order_ms;    /* k_mixed_order: the packages regrouped by sample rate (device time) */
 } r433b_timing;
 
 int r433b_create(int cuda_device, r433b_ctx **out);
@@ -198,6 +200,35 @@ int r433b_set_gates(r433b_ctx *ctx, r433b_gate const *gates, uint32_t n);
 /* rtl_433 -r on every stream of the batch: block loop, flush, reset (src/rtl_433.c:1797-1854),
    then all slicers on every package.  Synchronous; results stay on the device until fetched. */
 int r433b_process(r433b_ctx *ctx, r433b_batch const *batch);
+/* ---- mixed batches: capture files of different sample formats, rates and centre frequencies in one batch ----------
+   `rtl_433 -r f1 -r f2 ...` takes its files one after another and sets the sample size, rate and FPDM at each file
+   (src/rtl_433.c:1703-1745).  r433b_process_mixed() does the same for a batch whose stream i is described by fmt[i];
+   the results are those of r433b_process() on each file alone, in the caller's stream order.
+   - The batch's sample_format, samp_rate and center_frequency must be 0 (R433B_EINVAL otherwise).  fpdm_mode,
+     block_bytes, lengths and data_on_device keep their meaning; R433B_FPDM_AUTO is resolved per stream from its centre
+     frequency.  block_bytes must be a whole number of tiles for every sample size present.
+   - Per stream: the rate is not 0; the offset is a multiple of 16 bytes (32 for cf32).  Without lengths the offsets
+     ascend and stream i fills its gap; with lengths, stream i is [offsets[i], offsets[i] + lengths[i]), which must end by
+     offsets[n_streams], and the offsets need not ascend.
+   - want_stages returns R433B_EINVAL.  There is no chained (r433b_process_chained) and no asynchronous (r433b_submit)
+     form.  A mixed batch runs unsplit whatever r433b_set_split says, and host input goes to the device in one copy,
+     without time slices (r433b_set_pipeline).
+   - Streams that one detector launch can walk together (the same sample size after load-time conversion, cs8 flip,
+     rate and resolved FPDM) form a class.  Each class is one launch of k_front and k_detect; the launches run
+     side by side on a small pool of CUDA streams.  r433b_timing: front_ms is the wall time from the first launch to
+     the end of the last k_front, detect_ms from the start of the first k_detect to the end of the last; mixed_classes
+     counts the classes, detect_launches the launches (a class whose streams lie in two device buffers, the caller's
+     and that of the converted cf32 streams, takes one per buffer).
+   - Afterwards everything works as after r433b_process(), and every value refers to the stream's own format, rate and
+     centre frequency: fetch, digests, r433b_package_to_pulse_data(), r433b_package_file_pos(), the dispatch calls,
+     the analyzer and the grabber.  The grabber's run is every stream's used bytes in the caller's order, so a window
+     may reach back into an earlier file of another sample size, as the reference's does. */
+typedef struct r433b_stream_format {
+    uint32_t sample_format;    /* R433B_FMT_CU8 / _CS8 / _CS16 / _CF32 */
+    uint32_t samp_rate;        /* Hz, != 0 */
+    uint32_t center_frequency; /* Hz */
+} r433b_stream_format;
+int r433b_process_mixed(r433b_ctx *ctx, r433b_batch const *batch, r433b_stream_format const *fmt /* n_streams */);
 /* ---- chained batches: files longer than one batch, corpora larger than memory, buffers as they arrive ----------
    The reference pushes a file through push_sdr_flow() one block at a time and carries O(1) state between the calls
    (src/rtl_433.c:1827).  A chain does the same for the streams of consecutive batches: slot i of the chain carries the

@@ -20,6 +20,9 @@
   frequency) group in command-line order, groups in the order their first file appears.  That is the
   command-line order unless groups interleave.  The modes unknown / known / undecoded depend on what the
   decoders return, so they live behind r433b_dispatch (INTEGRATION.md), not here.
+* `--one-batch` replays every file in one mixed batch (r433b_process_mixed), each with its own format, rate and
+  frequency, in command-line order: the report is the same, and the files `-S all` writes are those of
+  `rtl_433 -S all -r f1 -r f2 ...` whatever the groups.  It does not combine with `--chunk-mb` or `--split`.
 
 Decoding itself stays with the reference's decoders (INTEGRATION.md); this module stops at the
 bitbuffer like the rest of the package.
@@ -170,13 +173,18 @@ def read_sigmf(path):
 _ABI_FORMAT = {"cu8": lib.FMT_CU8, "cs8": lib.FMT_CS8, "cs16": lib.FMT_CS16, "cf32": lib.FMT_CF32}
 
 
-def load_batches(specs, default_rate=DEFAULT_RATE, default_freq=DEFAULT_FREQ, uniform="auto"):
+def load_batches(specs, default_rate=DEFAULT_RATE, default_freq=DEFAULT_FREQ, uniform="auto", one_batch=False):
     """-> list of dict(format, sample_rate, center_frequency, files, data, offsets, lengths), one per
     (format, rate, frequency) group, files in command-line order inside a group.
 
     `uniform`: put the files of a group on ONE stride (the longest file, rounded up) so that r433b_process() can
     overlap the host-to-device copy with the kernels, time slice by time slice (one strided copy per slice);
-    "auto" does it when the padding costs less than half again the bytes, False packs the files back to back."""
+    "auto" does it when the padding costs less than half again the bytes, False packs the files back to back.
+
+    one_batch: ONE batch of every file in command-line order, packed back to back at 32-byte aligned starts, for
+    r433b_process_mixed: format "mixed", and per file "formats" (names), "abi_formats", "rates" and "freqs"."""
+    if one_batch:
+        return [_mixed_batch(specs, default_rate, default_freq)]
     groups = {}
     preloaded = {}
     for spec in specs:
@@ -212,6 +220,34 @@ def load_batches(specs, default_rate=DEFAULT_RATE, default_freq=DEFAULT_FREQ, un
     return out
 
 
+def _mixed_batch(specs, default_rate=DEFAULT_RATE, default_freq=DEFAULT_FREQ):
+    files, fmts, rates, freqs, bufs = [], [], [], [], []
+    for spec in specs:
+        info = parse_capture_name(spec)
+        if info["content"] == "sigmf":
+            sm = read_sigmf(info["path"])
+            fmt, rate, freq, buf = "cu8", sm["sample_rate"], sm["center_frequency"], sm["data"]
+        else:
+            if info["format"] not in _ABI_FORMAT:
+                raise ValueError(f"{spec}: format {info['format']!r} is not on the GPU path (cu8, cs8, cs16, cf32 are)")
+            fmt, rate = info["format"], info["sample_rate"] or default_rate
+            freq, buf = info["center_frequency"] or default_freq, np.fromfile(info["path"], dtype=np.uint8)
+        files.append(info["path"])
+        fmts.append(fmt)
+        rates.append(rate)
+        freqs.append(freq)
+        bufs.append(buf)
+    lengths = np.array([len(b) // _IN_BYTES[_ABI_FORMAT[f]] * _IN_BYTES[_ABI_FORMAT[f]] for b, f in zip(bufs, fmts)], np.uint64)
+    offsets = np.zeros(len(bufs) + 1, np.uint64)
+    for i, n in enumerate(lengths):
+        offsets[i + 1] = offsets[i] + (int(n) + 31) // 32 * 32
+    data = np.zeros(int(offsets[-1]), np.uint8)
+    for i, b in enumerate(bufs):
+        data[int(offsets[i]):int(offsets[i]) + int(lengths[i])] = b[:int(lengths[i])]
+    return {"format": "mixed", "files": files, "formats": fmts, "abi_formats": [_ABI_FORMAT[f] for f in fmts],
+            "rates": rates, "freqs": freqs, "data": data, "offsets": offsets, "lengths": lengths}
+
+
 def row_code(bb, row):
     """rtl_433's '{len}hex' row notation (src/decoder_util.c:61-90) of a re-inflated bitbuffer record."""
     n = int(bb["bits_per_row"][row])
@@ -240,8 +276,9 @@ class Grabber:
         self.counter = 1  # samp_grab_create()
         self.ring = None  # (bytes pushed, tail)
 
-    def write(self, ctx, mode, center_frequency, samp_rate, sample_size):
-        """Write the batch's files; -> their names."""
+    def write(self, ctx, mode, center_frequency, samp_rate, sample_size, per_stream=None):
+        """Write the batch's files; -> their names.  per_stream: (center_frequency, samp_rate, sample_size) of every
+        stream of a mixed batch, which then name each grab from the stream whose block call ended its frame."""
         prior = None if self.ring is None else (self.ring[0], self.ring[1], self.counter)
         plan = ctx.grab_plan(mode, prior)
         names = []
@@ -255,7 +292,8 @@ class Grabber:
             at = 0
             for g in plan[i:j]:
                 n = int(g["bytes"])
-                names.append(self._file(data[at:at + n], int(g["grab_len"]), center_frequency, samp_rate, sample_size))
+                fmt = (center_frequency, samp_rate, sample_size) if per_stream is None else per_stream[int(g["stream"])]
+                names.append(self._file(data[at:at + n], int(g["grab_len"]), *fmt))
                 at += n
             i = j
         self.ring = ctx.grab_tail()
@@ -373,11 +411,31 @@ def _replay_chunked(ctx, batch, chunk_mb, report):
     return reps
 
 
-def replay(specs, protocols=None, cuda_device=0, max_rows=8, out=print, grab_mode=0, grab_dir=".", chunk_mb=0, split=0):
+def _replay_mixed(ctx, grabber, grab_mode, batch, report, out):
+    """Every file in one mixed batch; the report in command-line order."""
+    ctx.process_mixed(batch["data"], batch["offsets"], batch["abi_formats"], batch["rates"], batch["freqs"],
+                      lengths=batch["lengths"])
+    res = ctx.fetch()
+    if grabber:
+        ss = {"cu8": 2, "cs8": 2, "cs16": 4, "cf32": 4}
+        grabber.write(ctx, grab_mode, None, None, None,
+                      per_stream=[(f, r, ss[t]) for f, r, t in zip(batch["freqs"], batch["rates"], batch["formats"])])
+    summary = []
+    for i, path in enumerate(batch["files"]):
+        one = {"format": batch["formats"][i], "sample_rate": batch["rates"][i], "center_frequency": batch["freqs"][i]}
+        n_samples = int(batch["lengths"][i]) // _IN_BYTES[batch["abi_formats"][i]]
+        summary.append(_print_file(out, path, one, n_samples, report(res, i)))
+    return summary
+
+
+def replay(specs, protocols=None, cuda_device=0, max_rows=8, out=print, grab_mode=0, grab_dir=".", chunk_mb=0, split=0,
+           one_batch=False):
     """Run capture files through the GPU path; report packages and slicer output per file.  grab_mode 1 writes
     every frame's IQ to grab_dir (`-S all`).  chunk_mb > 0 streams every group through a chain, chunk_mb MiB of every
     file per call: the report is the same, host memory stays bounded.  split (blocks per segment, or lib.SPLIT_AUTO)
-    walks long files in segments on separate warps: the report is the same, long files finish sooner."""
+    walks long files in segments on separate warps: the report is the same, long files finish sooner.  one_batch
+    replays every file in one mixed batch in command-line order (r433b_process_mixed): the report is the same, and
+    -S all writes what the reference writes for the files in that order."""
     table = lib.default_device_table(include_disabled=True)
     if protocols:
         devs = [d for d in table if d["protocol_num"] in set(protocols)]
@@ -389,6 +447,8 @@ def replay(specs, protocols=None, cuda_device=0, max_rows=8, out=print, grab_mod
         raise ValueError("the signal grabber does not run on chained batches (-S with --chunk-mb)")
     if split and chunk_mb:
         raise ValueError("segmented replay does not run on chained batches (--split with --chunk-mb)")
+    if one_batch and (chunk_mb or split):
+        raise ValueError("a mixed batch runs neither chained (--chunk-mb) nor split (--split)")
     ctx = lib.Context(cuda_device)
     ctx.set_devices(devs)
     if split:
@@ -396,6 +456,9 @@ def replay(specs, protocols=None, cuda_device=0, max_rows=8, out=print, grab_mod
     grabber = Grabber(grab_dir) if grab_mode else None
     summary = []
     try:
+        if one_batch:
+            return _replay_mixed(ctx, grabber, grab_mode, load_batches(specs, one_batch=True)[0],
+                                 lambda res, i: _file_rows(ctx, res, i, devs, protocols, max_rows), out)
         groups = _chunked_groups(specs) if chunk_mb else load_batches(specs)
         for batch in groups:
             if chunk_mb:
@@ -428,6 +491,8 @@ def main(argv=None):
                     help="stream every file through a chain, N MiB of whole blocks per call (bounded host memory)")
     ap.add_argument("--split", nargs="?", const="auto", default=None, metavar="N|auto",
                     help="walk long files in segments of N blocks on separate warps (auto: sized from the batch)")
+    ap.add_argument("--one-batch", action="store_true",
+                    help="every file in one mixed batch, each with its own format, rate and frequency, in command-line order")
     a = ap.parse_args(argv)
     split = 0
     if a.split is not None:
@@ -443,8 +508,10 @@ def main(argv=None):
         ap.error("--chunk-mb must be positive")
     if a.grab and a.chunk_mb:
         ap.error("-S does not run with --chunk-mb: the signal grabber does not run on chained batches")
+    if a.one_batch and (a.chunk_mb or a.split is not None):
+        ap.error("--one-batch does not run with --chunk-mb or --split: a mixed batch runs neither chained nor split")
     replay(a.files, a.protocols, a.device, grab_mode=lib.GRAB_ALL if a.grab else 0, grab_dir=a.grab_dir,
-           chunk_mb=a.chunk_mb, split=split)
+           chunk_mb=a.chunk_mb, split=split, one_batch=a.one_batch)
 
 
 if __name__ == "__main__":

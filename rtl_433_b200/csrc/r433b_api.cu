@@ -13,6 +13,7 @@
 #include <mutex>
 #include <string>
 #include <thread>
+#include <tuple>
 #include <vector>
 
 #include "../../include/r433b.h"
@@ -24,6 +25,7 @@
 #include "r433b_analyze_host.hpp"
 #include "r433b_grab.cuh"
 #include "r433b_split.cuh"
+#include "r433b_mixed.cuh"
 
 using namespace r433b;
 
@@ -150,6 +152,17 @@ struct r433b_ctx {
     int spoil_seed = 0;
     DevBuf d_sp_state, d_sp_train, d_sp_seed, d_sp_seed_train, d_sp_rw_state, d_sp_rw_train;
     DevBuf d_sp_view, d_sp_flags, d_sp_list, d_sp_eq, d_sp_tab, d_sp_pkgs, d_sp_ppool, d_sp_gpool;
+    // mixed batches (r433b_process_mixed): per caller stream its sample size, rate, centre frequency, and where its bytes
+    // (cf32: converted to cs16) lie on the device with the flip they are read with; empty for every other batch
+    struct MixedStream {
+        uint32_t SS, rate, center, flip;
+        uint8_t const *src;
+    };
+    std::vector<MixedStream> mixed;
+    static constexpr int kMixedStreams = 4; // the CUDA streams the class launches go round-robin onto
+    cudaStream_t s_mx[kMixedStreams]{};
+    std::vector<cudaEvent_t> ev_mx;         // per launch: k_front done, k_detect done
+    DevBuf d_mx_tab, d_mx_pkgs;
 };
 
 // What must not change while a chain has an open file: everything the carried state depends on
@@ -233,6 +246,18 @@ int fail(r433b_ctx *c, int code, char const *what, cudaError_t e = cudaSuccess)
 // cs8 is read as cu8: the load-time +128 of src/rtl_433.c:1830-1834 is an XOR of every byte's sign bit
 unsigned dp_flip_of(uint32_t sample_format) { return sample_format == R433B_FMT_CS8 ? 0x80808080u : 0u; }
 
+// What the host replay reads of a stream's format: bytes per sample (dm_state.sample_size), rate, centre frequency.  A
+// mixed batch has them per stream, every other batch once.
+struct StreamFormat {
+    uint32_t SS, rate, center;
+};
+StreamFormat stream_format(r433b_ctx const *ctx, uint32_t s)
+{
+    if (ctx->mixed.empty()) return {ctx->batch.sample_format, ctx->batch.samp_rate, ctx->batch.center_frequency};
+    r433b_ctx::MixedStream const &m = ctx->mixed[s];
+    return {m.SS, m.rate, m.center};
+}
+
 int dev_reserve(r433b_ctx *ctx, DevBuf &b, size_t bytes)
 {
     if (bytes <= b.cap) return 0;
@@ -299,6 +324,7 @@ int r433b_create(int cuda_device, r433b_ctx **out)
     cudaStreamCreateWithFlags(&ctx->s_in, cudaStreamNonBlocking);
     cudaStreamCreateWithFlags(&ctx->s_det, cudaStreamNonBlocking);
     cudaStreamCreateWithFlags(&ctx->s_out, cudaStreamNonBlocking);
+    for (auto &v : ctx->s_mx) cudaStreamCreateWithFlags(&v, cudaStreamNonBlocking);
     for (auto &v : ctx->ev_in) cudaEventCreateWithFlags(&v, cudaEventDisableTiming);
     for (auto &v : ctx->ev_det) cudaEventCreateWithFlags(&v, cudaEventDisableTiming);
     for (auto &v : ctx->ev_slc) cudaEventCreateWithFlags(&v, cudaEventDisableTiming);
@@ -335,7 +361,7 @@ void r433b_destroy(r433b_ctx *ctx)
                  &ctx->d_grab_prior, &ctx->d_grab_segs, &ctx->d_grab_stage, &ctx->d_sp_state, &ctx->d_sp_train,
                  &ctx->d_sp_seed, &ctx->d_sp_seed_train, &ctx->d_sp_rw_state, &ctx->d_sp_rw_train, &ctx->d_sp_view,
                  &ctx->d_sp_flags, &ctx->d_sp_list, &ctx->d_sp_eq, &ctx->d_sp_tab, &ctx->d_sp_pkgs, &ctx->d_sp_ppool,
-                 &ctx->d_sp_gpool})
+                 &ctx->d_sp_gpool, &ctx->d_mx_tab, &ctx->d_mx_pkgs})
         if (b->p) cudaFree(b->p);
     for (HostBuf *b : {&ctx->h_pkgs, &ctx->h_ppool, &ctx->h_gpool, &ctx->h_pairs, &ctx->h_events, &ctx->h_ranges})
         if (b->p) cudaFreeHost(b->p);
@@ -349,7 +375,10 @@ void r433b_destroy(r433b_ctx *ctx)
     for (auto &v : ctx->ev_f)
         if (v) cudaEventDestroy(v);
     if (ctx->ev_init) cudaEventDestroy(ctx->ev_init);
+    for (auto &v : ctx->ev_mx) cudaEventDestroy(v);
     for (cudaStream_t st : {ctx->s_in, ctx->s_det, ctx->s_out})
+        if (st) cudaStreamDestroy(st);
+    for (cudaStream_t st : ctx->s_mx)
         if (st) cudaStreamDestroy(st);
     delete ctx;
 }
@@ -628,6 +657,7 @@ int adopt_batch(r433b_ctx *ctx, r433b_batch const *b, Shape &s)
     ctx->processed = ctx->fetched = false;
     ctx->chained = ctx->pulse_mode = false;
     ctx->chain_last = nullptr;
+    ctx->mixed.clear();
     ctx->batch = *b;
     ctx->batch.sample_format = (uint32_t)s.SS; // the host replay only needs the sample size (dm_state.sample_size)
     ctx->batch.block_bytes = s.settings.block_bytes;
@@ -650,6 +680,18 @@ int adopt_batch(r433b_ctx *ctx, r433b_batch const *b, Shape &s)
     ctx->timing.grab_ms = ctx->timing.grab_ring_ms = 0;
     ctx->d2h_done = false;
     return R433B_OK;
+}
+
+// The FM low-pass of a launch from its sample size, rate, FPDM and whether FM is on
+void set_fm_filter(r433b_ctx const *ctx, int SS, DetectParams &dp)
+{
+    dp.wrap_free = 1;
+    if (dp.enable_fm) {
+        float lp = ctx->fm_low_pass != 0.0f ? ctx->fm_low_pass : dp.fpdm ? 0.2f : 0.1f; // src/r_flow.c:204
+        fm_coeffs(SS == 4, dp.rate, lp, dp.fm_a1, dp.fm_b0);
+        long long unity = SS == 2 ? 16384ll : (1ll << 30);
+        dp.wrap_free = dp.fm_a1 >= 0 && dp.fm_b0 >= 0 && (long long)dp.fm_a1 + 2ll * dp.fm_b0 <= unity;
+    }
 }
 
 // The device buffers of the batch (no data moved yet) and the detector's launch parameters, into a zeroed `dp`
@@ -702,13 +744,7 @@ int prepare_detect(r433b_ctx *ctx, r433b_batch const *b, Shape const &s, DetectP
     dp.lv = ctx->lv;
     dp.lpf_a1 = ((int)(0.85408 * 32768)) >> 1; // src/baseband.c:151-152
     dp.lpf_b0 = ((int)(0.07296 * 32768)) >> 1;
-    dp.wrap_free = 1;
-    if (dp.enable_fm) {
-        float lp = ctx->fm_low_pass != 0.0f ? ctx->fm_low_pass : dp.fpdm ? 0.2f : 0.1f; // src/r_flow.c:204
-        fm_coeffs(SS == 4, b->samp_rate, lp, dp.fm_a1, dp.fm_b0);
-        long long unity = SS == 2 ? 16384ll : (1ll << 30);
-        dp.wrap_free = dp.fm_a1 >= 0 && dp.fm_b0 >= 0 && (long long)dp.fm_a1 + 2ll * dp.fm_b0 <= unity;
-    }
+    set_fm_filter(ctx, SS, dp);
     dp.train_scratch = (int *)ctx->d_train.p;
     dp.log_scratch = (unsigned *)ctx->d_log.p;
     dp.counters = (DetectCounters *)ctx->d_counters.p;
@@ -776,18 +812,19 @@ int chain_finish(r433b_ctx *ctx, r433b_chain *ch, uint8_t const *last, Shape con
     return chain_grab_append(ctx, ch);
 }
 
-// k_front over the tiles [sample_begin, sample_end) of every stream, then the walk over the same range
+// k_front over the tiles [sample_begin, sample_end) of the streams [stream0, stream_end), then the walk over the same range
 void launch_detect(r433b_ctx *ctx, DetectParams const &q, Shape const &s, cudaStream_t st, cudaEvent_t after_front)
 {
     int const SS = s.SS, T = kTile;
+    unsigned const n_launch = q.stream_end - q.stream0;
     uint64_t const t_end = (std::min<uint64_t>(q.sample_end, s.max_samples) + T - 1) / T, t_begin = q.sample_begin / T;
     if (t_end > t_begin) {
         FrontParams fp{};
         fp.data = q.data;
-        fp.offsets = q.offsets;
-        fp.lengths = q.lengths;
-        fp.am_offsets = q.am_offsets;
-        fp.n_streams = q.n_streams;
+        fp.offsets = q.offsets + q.stream0;
+        fp.lengths = q.lengths ? q.lengths + q.stream0 : nullptr;
+        fp.am_offsets = q.am_offsets + q.stream0;
+        fp.n_streams = n_launch;
         fp.tile_begin = t_begin;
         fp.tiles = (unsigned)(t_end - t_begin);
         fp.use_mag = q.use_mag;
@@ -800,16 +837,16 @@ void launch_detect(r433b_ctx *ctx, DetectParams const &q, Shape const &s, cudaSt
         fp.tile_info = (TileInfo *)ctx->d_tiles.p;
         fp.counters = q.counters;
         fp.spoil = ctx->spoil_front;
-        fp.state = q.state;
-        fp.cont = q.first_chunk ? q.cont : nullptr;
-        uint64_t const warps = (uint64_t)q.n_streams * fp.tiles;
+        fp.state = q.state ? q.state + q.stream0 : nullptr;
+        fp.cont = q.first_chunk && q.cont ? q.cont + q.stream0 : nullptr;
+        uint64_t const warps = (uint64_t)n_launch * fp.tiles;
         unsigned const fgrid = (unsigned)((warps + kFrontWarps - 1) / kFrontWarps);
         void (*ffn)(FrontParams) = SS == 2 ? k_front<2> : k_front<4>;
         size_t const fsm = (size_t)kFrontWarps * (SS == 2 ? FrontStage<2>::kBytes : FrontStage<4>::kBytes);
         R4_LAUNCH(ffn, fgrid, kFrontWarps * 32, fsm, st, fp);
     }
     cudaEventRecord(after_front, st);
-    unsigned grid = (q.n_streams + kDetectWarps - 1) / kDetectWarps;
+    unsigned grid = (n_launch + kDetectWarps - 1) / kDetectWarps;
     size_t sm = (size_t)kDetectWarps * sizeof(WarpSmem);
     void (*kfn)(DetectParams) = SS == 2 ? k_detect<2> : k_detect<4>;
     R4_LAUNCH(kfn, grid, kDetectWarps * 32, sm, st, q);
@@ -1396,6 +1433,8 @@ int process_iq(r433b_ctx *ctx, r433b_batch const *b, r433b_chain *ch, uint8_t co
     ctx->arena_cap = std::max<size_t>(ctx->arena_cap, ctx->min_caps[2] ? ctx->min_caps[2] : s.total_bytes / 2 + (1u << 20));
     ctx->timing.split_segments = ctx->timing.split_rewalks = ctx->timing.split_rounds = 0;
     ctx->timing.split_merge_ms = 0;
+    ctx->timing.mixed_classes = 0;
+    ctx->timing.mixed_order_ms = 0;
     DetectCounters cnt{};
     int r = kFellBack;
     SplitPlan plan;
@@ -1423,9 +1462,288 @@ int process_iq(r433b_ctx *ctx, r433b_batch const *b, r433b_chain *ch, uint8_t co
     return chain_finish(ctx, ch, last, s);
 }
 
+// ---- mixed batches (r433b_process_mixed, DESIGN §7d) -----------------------------------------------------------------
+
+// A class: the streams one detector launch can walk together, and the device buffer they lie in.  The internal order
+// sorts the streams by class, stable in the caller's; a class is the internal streams [begin, end).
+struct MixedClass {
+    uint32_t rate, SS, flip, fpdm, buf;
+    uint32_t begin, end;
+    uint64_t max_samples;
+    bool same(MixedClass const &o) const
+    {
+        return rate == o.rate && SS == o.SS && flip == o.flip && fpdm == o.fpdm && buf == o.buf;
+    }
+};
+
+// rtl_433 -r f1 -r f2 ... on a batch of files of their own formats: one k_front + k_detect launch per class on the
+// CUDA stream pool, k_mixed_order, then the slicers over one package range per rate.
+int process_mixed(r433b_ctx *ctx, r433b_batch const *b, r433b_stream_format const *fmt)
+{
+    if (!ctx || !b || !b->offsets || (b->n_streams && (!b->data || !fmt))) return fail(ctx, R433B_EINVAL, "null argument");
+    if (b->sample_format || b->samp_rate || b->center_frequency)
+        return fail(ctx, R433B_EINVAL, "r433b_process_mixed: the batch's sample_format, samp_rate and center_frequency "
+                                       "must be 0 (each stream has its own)");
+    if (b->want_stages) return fail(ctx, R433B_EINVAL, "r433b_process_mixed: no stage arrays (want_stages)");
+    uint32_t const n = b->n_streams;
+    uint32_t const block_bytes = b->block_bytes ? b->block_bytes : 262144u;
+    uint64_t const total = n ? b->offsets[n] : 0;
+    if (total % 16) return fail(ctx, R433B_EINVAL, "offsets[n_streams] must be a multiple of 16 bytes");
+    int enable_fm = 0;
+    for (auto const &d : ctx->devs)
+        if (d.modulation >= 16) enable_fm = 1;
+    // per stream: checks, its class key, its bytes after conversion (cf32 -> cs16, in the conversion region)
+    std::vector<MixedClass> key(n);
+    std::vector<uint64_t> len(n), conv(n, UINT64_MAX);
+    uint64_t conv_bytes = 0;
+    for (uint32_t i = 0; i < n; ++i) {
+        uint32_t const f = fmt[i].sample_format;
+        if (f != R433B_FMT_CU8 && f != R433B_FMT_CS16 && f != R433B_FMT_CS8 && f != R433B_FMT_CF32)
+            return fail(ctx, R433B_EINVAL, "sample_format must be R433B_FMT_CU8, _CS8, _CS16 or _CF32");
+        if (fmt[i].samp_rate == 0) return fail(ctx, R433B_EINVAL, "samp_rate is 0");
+        uint32_t const SS = f & 0xff, in_div = f == R433B_FMT_CF32 ? 2 : 1;
+        if (block_bytes % (uint32_t)(kTile * SS) != 0)
+            return fail(ctx, R433B_EINVAL, "block_bytes must be a multiple of 2048 samples of every sample size in the batch");
+        if (b->offsets[i] % (16 * in_div)) return fail(ctx, R433B_EINVAL, "stream offsets must be multiples of 16 bytes (32 for cf32)");
+        uint64_t const in_len = b->lengths ? b->lengths[i] : b->offsets[i + 1] - b->offsets[i];
+        if (!b->lengths && b->offsets[i + 1] < b->offsets[i]) return fail(ctx, R433B_EINVAL, "offsets not ascending");
+        if (b->offsets[i] > total || in_len > total - b->offsets[i])
+            return fail(ctx, R433B_EINVAL, "a stream ends behind offsets[n_streams]");
+        len[i] = in_div == 2 ? in_len / 8 * 4 : in_len; // whole IQ pairs of floats -> cs16 bytes
+        if (in_div == 2) {
+            conv[i] = conv_bytes;
+            conv_bytes += (len[i] + 15) / 16 * 16;
+        }
+        uint32_t const fpdm = b->fpdm_mode == R433B_FPDM_AUTO ? (fmt[i].center_frequency > 800000000u ? 1u : 0u) : b->fpdm_mode;
+        key[i] = MixedClass{fmt[i].samp_rate, SS, dp_flip_of(f), fpdm, in_div == 2 && b->data_on_device ? 1u : 0u, 0, 0, 0};
+    }
+    CU(cudaSetDevice(ctx->device));
+
+    // the batch becomes the context's last one
+    ctx->processed = ctx->fetched = false;
+    ctx->chained = ctx->pulse_mode = false;
+    ctx->chain_last = nullptr;
+    ctx->batch = *b;
+    ctx->batch.block_bytes = block_bytes;
+    ctx->grabs.clear();
+    ctx->grab_planned = false;
+    ctx->grab_src = nullptr;
+    ctx->grab_flip = 0;
+    ctx->timing = r433b_timing{};
+    ctx->d2h_done = false;
+    // device buffers: host input is copied whole to d_data; the converted cf32 streams follow it there (host input) or
+    // fill it (device input)
+    uint64_t const conv_base = b->data_on_device ? 0 : (total + 255) / 256 * 256;
+    if (!b->data_on_device || conv_bytes)
+        if (int r = dev_reserve(ctx, ctx->d_data, conv_base + conv_bytes + 64)) return r;
+    uint8_t const *const caller = b->data_on_device ? (uint8_t const *)b->data : (uint8_t const *)ctx->d_data.p;
+    uint8_t const *const region = (uint8_t const *)ctx->d_data.p;
+    ctx->offsets.assign(n + 1, total);
+    ctx->lengths = len;
+    ctx->mixed.resize(n);
+    uint64_t used = 0, n_samples = 0;
+    for (uint32_t i = 0; i < n; ++i) {
+        bool const cv = conv[i] != UINT64_MAX;
+        ctx->offsets[i] = cv ? conv_base + conv[i] : b->offsets[i];
+        ctx->mixed[i] = r433b_ctx::MixedStream{key[i].SS, fmt[i].samp_rate, fmt[i].center_frequency, key[i].flip,
+                                               cv ? region : caller};
+        used += len[i];
+        n_samples += len[i] / key[i].SS;
+    }
+    ctx->batch.offsets = ctx->offsets.data();
+    ctx->batch.lengths = ctx->lengths.data();
+
+    // the internal order and the classes; the device reads the offsets, lengths and AM offsets in that order
+    std::vector<uint32_t> order(n);
+    for (uint32_t i = 0; i < n; ++i) order[i] = i;
+    auto less = [&](MixedClass const &x, MixedClass const &y) {
+        return std::tie(x.rate, x.SS, x.flip, x.fpdm, x.buf) < std::tie(y.rate, y.SS, y.flip, y.fpdm, y.buf);
+    };
+    std::stable_sort(order.begin(), order.end(), [&](uint32_t x, uint32_t y) { return less(key[x], key[y]); });
+    std::vector<MixedClass> classes;
+    std::vector<uint32_t> rates, slot_first; // distinct rates ascending, and the first internal stream of each
+    std::vector<uint64_t> view(3 * n + 2);   // offsets (n + 1), lengths, AM offsets (n + 1)
+    uint64_t *off = view.data(), *lens = off + n + 1, *amoff = lens + n;
+    std::vector<uint32_t> caller_of(order);
+    amoff[0] = 0;
+    for (uint32_t j = 0; j < n; ++j) {
+        uint32_t const i = order[j];
+        if (classes.empty() || !classes.back().same(key[i])) {
+            classes.push_back(key[i]);
+            classes.back().begin = j;
+        }
+        if (rates.empty() || rates.back() != key[i].rate) {
+            rates.push_back(key[i].rate);
+            slot_first.push_back(j);
+        }
+        classes.back().end = j + 1;
+        classes.back().max_samples = std::max<uint64_t>(classes.back().max_samples, len[i] / key[i].SS);
+        off[j] = ctx->offsets[i];
+        lens[j] = len[i];
+        amoff[j + 1] = amoff[j] + (len[i] / key[i].SS + kTile - 1) / kTile * kTile;
+    }
+    off[n] = 0;
+    slot_first.push_back(n);
+    uint32_t n_classes = 0;
+    for (size_t c = 0; c < classes.size(); ++c)
+        n_classes += c == 0 || !(classes[c].rate == classes[c - 1].rate && classes[c].SS == classes[c - 1].SS
+                                 && classes[c].flip == classes[c - 1].flip && classes[c].fpdm == classes[c - 1].fpdm);
+    uint64_t const am_samples = amoff[n];
+    size_t const nn = std::max<size_t>(1, n);
+    if (int r = dev_reserve(ctx, ctx->d_offsets, (n + 1) * sizeof(uint64_t))) return r;
+    if (int r = dev_reserve(ctx, ctx->d_lengths, nn * sizeof(uint64_t))) return r;
+    if (int r = dev_reserve(ctx, ctx->d_amoff, (n + 1) * sizeof(uint64_t))) return r;
+    if (int r = dev_reserve(ctx, ctx->d_train, nn * kTrainInts * sizeof(int))) return r;
+    if (int r = dev_reserve(ctx, ctx->d_log, nn * kLogCap * 2 * sizeof(unsigned))) return r;
+    if (int r = dev_reserve(ctx, ctx->d_counters, 64)) return r;
+    if (int r = dev_reserve(ctx, ctx->d_am, am_samples * sizeof(int16_t) + 16)) return r;
+    if (int r = dev_reserve(ctx, ctx->d_chunks, am_samples / kChunk * sizeof(ChunkInfo) + 16)) return r;
+    if (int r = dev_reserve(ctx, ctx->d_tiles, am_samples / kTile * sizeof(TileInfo) + 16)) return r;
+    if (int r = dev_reserve(ctx, ctx->d_mx_tab, (2 * n + 1) * sizeof(uint32_t))) return r;
+    CU(cudaMemcpy(ctx->d_offsets.p, off, (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice));
+    if (n) CU(cudaMemcpy(ctx->d_lengths.p, lens, n * sizeof(uint64_t), cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(ctx->d_amoff.p, amoff, (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice));
+    if (n) CU(cudaMemcpy(ctx->d_mx_tab.p, caller_of.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    if (int r = upload_slicer_tables(ctx, rates, 0)) return r;
+    ctx->pkg_cap = std::max<size_t>(ctx->pkg_cap, ctx->min_caps[0] ? ctx->min_caps[0] : (size_t)n * 16 + 1024);
+    ctx->pool_cap = std::max<size_t>(ctx->pool_cap, ctx->min_caps[1] ? ctx->min_caps[1] : ctx->pkg_cap * 128);
+    ctx->arena_cap = std::max<size_t>(ctx->arena_cap, ctx->min_caps[2] ? ctx->min_caps[2] : used / 2 + (1u << 20));
+
+    DetectParams dp{};
+    dp.offsets = (unsigned long long const *)ctx->d_offsets.p;
+    dp.lengths = (unsigned long long const *)ctx->d_lengths.p;
+    dp.am_offsets = (unsigned long long const *)ctx->d_amoff.p;
+    dp.n_streams = n;
+    dp.sample_end = ~0ull;
+    dp.first_chunk = 1;
+    dp.use_mag = ctx->use_mag;
+    dp.enable_fm = enable_fm;
+    dp.lv = ctx->lv;
+    dp.lpf_a1 = ((int)(0.85408 * 32768)) >> 1; // src/baseband.c:151-152
+    dp.lpf_b0 = ((int)(0.07296 * 32768)) >> 1;
+    dp.train_scratch = (int *)ctx->d_train.p;
+    dp.log_scratch = (unsigned *)ctx->d_log.p;
+    dp.counters = (DetectCounters *)ctx->d_counters.p;
+    dp.am = (int16_t *)ctx->d_am.p;
+    dp.chunks = (ChunkInfo const *)ctx->d_chunks.p;
+    dp.tile_info = (TileInfo const *)ctx->d_tiles.p;
+    size_t const n_launch = classes.size();
+    while (ctx->ev_mx.size() < 2 * n_launch) {
+        cudaEvent_t e;
+        CU(cudaEventCreate(&e));
+        ctx->ev_mx.push_back(e);
+    }
+
+    cudaStream_t const st = 0;
+    CU(cudaEventRecord(ctx->ev[0], st));
+    Shape whole{};
+    whole.total_bytes = total;
+    if (int r = copy_in(ctx, b, whole, st)) return r; // host input: one copy; device input: nothing
+    for (uint32_t i = 0; i < n; ++i) {
+        size_t const n4 = (size_t)(len[i] / 4 + 1) / 2; // two cs16 samples per group of four floats
+        if (conv[i] == UINT64_MAX || !n4) continue;
+        unsigned const grid = (unsigned)std::min<size_t>((size_t)ctx->n_sms * 8, (n4 + 255) / 256);
+        R4_LAUNCH(k_cf32_to_cs16, grid, 256, 0, st, (float4 const *)(caller + b->offsets[i]),
+                  (uint2 *)((uint8_t *)ctx->d_data.p + conv_base + conv[i]), n4);
+        CU(cudaGetLastError());
+    }
+    CU(cudaEventRecord(ctx->ev[1], st));
+    DetectCounters cnt{};
+    for (int attempt = 0;; ++attempt) {
+        if (int r = bind_detector_arenas(ctx, dp)) return r;
+        CU(cudaMemsetAsync(ctx->d_counters.p, 0, 64, st));
+        CU(cudaEventRecord(ctx->ev[4], st)); // the classes start here
+        for (size_t c = 0; c < n_launch; ++c) {
+            MixedClass const &k = classes[c];
+            cudaStream_t const ps = ctx->s_mx[c % r433b_ctx::kMixedStreams];
+            DetectParams q = dp;
+            q.data = k.buf ? region : caller;
+            q.stream0 = k.begin;
+            q.stream_end = k.end;
+            q.flip = k.flip;
+            q.fpdm = (int)k.fpdm;
+            q.rate = k.rate;
+            q.block_samples = block_bytes / k.SS;
+            set_fm_filter(ctx, (int)k.SS, q);
+            Shape sh{};
+            sh.SS = (int)k.SS;
+            sh.max_samples = k.max_samples;
+            CU(cudaStreamWaitEvent(ps, ctx->ev[4], 0));
+            launch_detect(ctx, q, sh, ps, ctx->ev_mx[2 * c]);
+            CU(cudaGetLastError());
+            CU(cudaEventRecord(ctx->ev_mx[2 * c + 1], ps));
+            CU(cudaStreamWaitEvent(st, ctx->ev_mx[2 * c + 1], 0));
+        }
+        CU(cudaMemcpyAsync(&cnt, ctx->d_counters.p, sizeof(cnt), cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        if (!cnt.overflow) break;
+        // arenas were too small: the counters hold the true need
+        ctx->pkg_cap = std::max<size_t>(ctx->pkg_cap, (size_t)cnt.pkgs + 64);
+        ctx->pool_cap = std::max<size_t>(ctx->pool_cap, (size_t)cnt.pool + 4096);
+        if (attempt == 2) return fail(ctx, R433B_EOVERFLOW, "package arena overflow");
+    }
+    if (int r = check_pair_index(ctx, cnt.pkgs)) return r;
+    ctx->n_pkgs = cnt.pkgs;
+    ctx->pool_used = cnt.pool;
+
+    // k_mixed_order: the headers by rate slot, with the caller's stream indices
+    std::vector<uint32_t> base(n + 1, 0);
+    if (int r = dev_reserve(ctx, ctx->d_mx_pkgs, ctx->pkg_cap * sizeof(r433b_package))) return r;
+    CU(cudaEventRecord(ctx->ev_t[0], st));
+    if (ctx->n_pkgs) {
+        MixedOrder mo{};
+        mo.src = (r433b_package const *)ctx->d_pkgs.p;
+        mo.dst = (r433b_package *)ctx->d_mx_pkgs.p;
+        mo.n_pkgs = ctx->n_pkgs;
+        mo.n_streams = n;
+        mo.caller = (unsigned const *)ctx->d_mx_tab.p;
+        mo.base = (unsigned *)ctx->d_mx_tab.p + n;
+        unsigned const grid = (unsigned)std::min<uint64_t>((uint64_t)ctx->n_sms * 4, (ctx->n_pkgs + kMixedThreads - 1) / kMixedThreads);
+        CU(cudaMemsetAsync(mo.base, 0, (n + 1) * sizeof(unsigned), st));
+        R4_LAUNCH(k_mixed_order, grid, kMixedThreads, 0, st, mo, 0);
+        R4_LAUNCH(k_mixed_order, 1, 32, 0, st, mo, 1);
+        R4_LAUNCH(k_mixed_order, grid, kMixedThreads, 0, st, mo, 2);
+        CU(cudaGetLastError());
+        CU(cudaMemcpyAsync(base.data(), mo.base, (n + 1) * sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+    }
+    CU(cudaEventRecord(ctx->ev_t[1], st));
+    CU(cudaEventSynchronize(ctx->ev_t[1]));
+    std::swap(ctx->d_pkgs, ctx->d_mx_pkgs);
+    std::vector<GroupRange> ranges(rates.size());
+    for (size_t g = 0; g < rates.size(); ++g) {
+        ranges[g].pkg_begin = base[slot_first[g]];
+        ranges[g].pkg_end = base[slot_first[g + 1]];
+    }
+    if (int r = slice_ranges(ctx, ranges, ctx->n_pkgs, ctx->pool_used, st)) return r;
+
+    auto ms = [](cudaEvent_t a, cudaEvent_t e) { float t = 0; cudaEventElapsedTime(&t, a, e); return t; };
+    float front_end = 0, detect_begin = 0, detect_end = 0;
+    for (size_t c = 0; c < n_launch; ++c) {
+        float const f = ms(ctx->ev[4], ctx->ev_mx[2 * c]), d = ms(ctx->ev[4], ctx->ev_mx[2 * c + 1]);
+        front_end = std::max(front_end, f);
+        detect_begin = c ? std::min(detect_begin, f) : f;
+        detect_end = std::max(detect_end, d);
+    }
+    ctx->timing.h2d_ms = ms(ctx->ev[0], ctx->ev[1]);
+    ctx->timing.front_ms = front_end;
+    ctx->timing.detect_ms = detect_end - detect_begin;
+    ctx->timing.total_ms = ms(ctx->ev[0], ctx->ev[3]);
+    ctx->timing.mixed_order_ms = ms(ctx->ev_t[0], ctx->ev_t[1]);
+    ctx->timing.mixed_classes = n_classes;
+    ctx->timing.detect_launches = ctx->timing.front_launches = (uint32_t)n_launch;
+    ctx->timing.front_redone = cnt.front_redone;
+    ctx->timing.front_repairs = cnt.front_repairs;
+    ctx->timing.idle_skipped = cnt.idle_skipped;
+    ctx->timing.idle_rewalks = cnt.idle_rewalks;
+    ctx->n_samples = n_samples;
+    ctx->processed = true;
+    return R433B_OK;
+}
+
 } // namespace
 
 int r433b_process(r433b_ctx *ctx, r433b_batch const *b) { return process_iq(ctx, b, nullptr, nullptr); }
+int r433b_process_mixed(r433b_ctx *ctx, r433b_batch const *b, r433b_stream_format const *fmt) { return process_mixed(ctx, b, fmt); }
 
 int r433b_chain_create(r433b_ctx *ctx, uint32_t n_streams, r433b_chain **out)
 {
@@ -1617,7 +1935,8 @@ float r433b_package_file_pos(r433b_ctx const *ctx, r433b_results const *res, uin
     if (!ctx || !res || package >= res->n_packages) return 0.0f;
     if (ctx->pulse_mode) return 0.0f; // demod->sample_file_pos = 0.0 in front of the .ook loop, src/rtl_433.c:1752
     r433b_package const &k = res->packages[package];
-    uint64_t SS = ctx->batch.sample_format;
+    StreamFormat const f = stream_format(ctx, k.stream);
+    uint64_t SS = f.SS;
     // a chained chunk: the bytes of its file up to the chunk's end (k.block is absolute)
     uint64_t bytes = ctx->lengths[k.stream] + (ctx->chained ? ctx->chain_base[k.stream] * SS : 0);
     uint32_t bb = ctx->batch.block_bytes;
@@ -1627,7 +1946,7 @@ float r433b_package_file_pos(r433b_ctx const *ctx, r433b_results const *res, uin
     // the flush keeps the last block's value
     uint64_t blk = (uint64_t)k.block < n_blocks ? (uint64_t)k.block : n_blocks - 1;
     unsigned long n_read = (unsigned long)std::min<uint64_t>(bb, bytes - blk * bb);
-    float pos = ((float)(int)blk * bb + n_read) / ctx->batch.samp_rate / (int)SS;
+    float pos = ((float)(int)blk * bb + n_read) / f.rate / (int)SS;
     return pos;
 }
 
@@ -1650,8 +1969,9 @@ int r433b_package_to_pulse_data(r433b_ctx const *ctx, r433b_results const *res, 
         pd->freq2_hz = m.freq2_hz;
         return R433B_OK;
     }
+    StreamFormat const f = stream_format(ctx, k.stream);
     pd->offset = k.offset;
-    pd->sample_rate = ctx->batch.samp_rate;
+    pd->sample_rate = f.rate;
     pd->start_ago = k.start_ago;
     pd->end_ago = k.end_ago;
     pd->num_pulses = k.num_pulses;
@@ -1667,14 +1987,14 @@ int r433b_package_to_pulse_data(r433b_ctx const *ctx, r433b_results const *res, 
     int const max_high = ctx->lv.max_high;
     float top = hi < max_high ? hi : max_high;
     float asnr = top / lo;
-    uint32_t rate = ctx->batch.samp_rate, center = ctx->batch.center_frequency;
+    uint32_t rate = f.rate, center = f.center;
     float off1 = (float)pd->fsk_f1_est / INT16_MAX * rate / 2.0f;
     float off2 = (float)pd->fsk_f2_est / INT16_MAX * rate / 2.0f;
     pd->freq1_hz = off1 + center;
     pd->freq2_hz = off2 + center;
     pd->centerfreq_hz = center;
-    pd->depth_bits = ctx->batch.sample_format * 4;
-    if (ctx->batch.sample_format == 2 && !ctx->use_mag) {
+    pd->depth_bits = f.SS * 4;
+    if (f.SS == 2 && !ctx->use_mag) {
         pd->range_db = 42.1442f;
         pd->rssi_db = 10.0f * log10f(hi) - 42.1442f;
         pd->noise_db = 10.0f * log10f(lo) - 42.1442f;
@@ -1949,6 +2269,7 @@ int r433b_process_pulses(r433b_ctx *ctx, r433b_pulses const *ps)
     ctx->pulse_mode = true;
     ctx->grab_planned = false;
     ctx->pulse_meta = set.pk;
+    ctx->mixed.clear();
     ctx->batch = r433b_batch{};
     ctx->batch.sample_format = 2;
     ctx->offsets.clear();
@@ -2026,7 +2347,7 @@ namespace {
 uint32_t package_rate(r433b_ctx const *ctx, r433b_package const &k)
 {
     if (ctx->pulse_mode && k.end_pos < ctx->pulse_meta.size()) return ctx->pulse_meta[k.end_pos].rate;
-    return ctx->batch.samp_rate;
+    return stream_format(ctx, k.stream).rate;
 }
 
 } // namespace
@@ -2218,14 +2539,16 @@ namespace {
 
 // The run byte range [a, b) as segments of the staging buffer from `dst` on: negative positions were never written
 // (zero), positions before the batch come from the device copy of the prior tail, the rest from the streams' used
-// bytes as they lie on the device.
-void grab_segments(r433b_ctx const *ctx, int64_t a, int64_t b, uint64_t &dst, std::vector<GrabSeg> &segs)
+// bytes as they lie on the device.  seg_stream gets each segment's stream (UINT32_MAX: not the batch's bytes).
+void grab_segments(r433b_ctx const *ctx, int64_t a, int64_t b, uint64_t &dst, std::vector<GrabSeg> &segs,
+        std::vector<uint32_t> &seg_stream)
 {
     int64_t const pushed = (int64_t)ctx->grab_pushed;
     while (a < b) {
         GrabSeg g{};
         g.dst = dst;
         int64_t e;
+        uint32_t stream = UINT32_MAX;
         if (a < 0) {
             e = std::min<int64_t>(b, 0);
             g.kind = kGrabZero;
@@ -2240,8 +2563,10 @@ void grab_segments(r433b_ctx const *ctx, int64_t a, int64_t b, uint64_t &dst, st
             e = std::min<int64_t>(b, pushed + (int64_t)cum[s + 1]);
             g.kind = kGrabBatch;
             g.src = ctx->offsets[s] + (u - cum[s]);
+            stream = (uint32_t)s;
         }
         g.len = (uint64_t)(e - a);
+        seg_stream.push_back(stream);
         segs.push_back(g);
         dst += g.len;
         a = e;
@@ -2283,18 +2608,20 @@ void chain_grab_segments(r433b_ctx const *ctx, r433b_chain const *ch, uint32_t s
     }
 }
 
-// k_grab over `segs` (covering [0, total)) into `out` (device, total rounded up to kGrabSpan)
-int grab_launch(r433b_ctx *ctx, std::vector<GrabSeg> const &segs, uint64_t total, uint8_t const *prior, void *out)
+// k_grab over `segs` (covering [0, total)) into `out` (device, total rounded up to kGrabSpan); the batch's bytes are
+// read from `batch` with `flip`
+int grab_launch(r433b_ctx *ctx, std::vector<GrabSeg> const &segs, uint64_t total, uint8_t const *batch, unsigned flip,
+        uint8_t const *prior, void *out)
 {
     cudaStream_t const st = 0;
     if (int r = dev_reserve(ctx, ctx->d_grab_segs, segs.size() * sizeof(GrabSeg))) return r;
     CU(cudaMemcpyAsync(ctx->d_grab_segs.p, segs.data(), segs.size() * sizeof(GrabSeg), cudaMemcpyHostToDevice, st));
     GrabParams gp{};
-    gp.batch = ctx->grab_src;
+    gp.batch = batch;
     gp.prior = prior;
     gp.segs = (GrabSeg const *)ctx->d_grab_segs.p;
     gp.n_segs = (unsigned)segs.size();
-    gp.flip = ctx->grab_flip;
+    gp.flip = flip;
     gp.total = total;
     gp.out = (uint4 *)out;
     uint64_t const warps = (total + kGrabSpan - 1) / kGrabSpan;
@@ -2304,19 +2631,62 @@ int grab_launch(r433b_ctx *ctx, std::vector<GrabSeg> const &segs, uint64_t total
     return R433B_OK;
 }
 
-// k_grab over `segs` (covering [0, total)) into the staging buffer, then one copy to `out`
-int grab_gather(r433b_ctx *ctx, std::vector<GrabSeg> const &segs, uint64_t total, uint8_t *out)
+// k_grab over `segs` (covering [0, total)) into the staging buffer, then one copy to `out`.  In a mixed batch the
+// streams' bytes lie in two buffers (the caller's, the converted cf32 streams') and cs8 alone is flipped: one k_grab per
+// (buffer, flip) gathers its segments into a region of its own, and the host puts every segment in its place.
+int grab_gather(r433b_ctx *ctx, std::vector<GrabSeg> const &segs, std::vector<uint32_t> const &seg_stream, uint64_t total,
+        uint8_t *out)
 {
     if (!total) return R433B_OK;
     cudaStream_t const st = 0;
-    uint64_t const staged = (total + kGrabSpan - 1) / kGrabSpan * kGrabSpan;
-    if (int r = dev_reserve(ctx, ctx->d_grab_stage, staged)) return r;
     void const *prior = ctx->chained ? ctx->chain_last->d_pre.p : ctx->d_grab_prior.p;
+    if (ctx->mixed.empty()) {
+        uint64_t const staged = (total + kGrabSpan - 1) / kGrabSpan * kGrabSpan;
+        if (int r = dev_reserve(ctx, ctx->d_grab_stage, staged)) return r;
+        CU(cudaEventRecord(ctx->ev[0], st));
+        if (int r = grab_launch(ctx, segs, total, ctx->grab_src, ctx->grab_flip, (uint8_t const *)prior, ctx->d_grab_stage.p)) return r;
+        CU(cudaEventRecord(ctx->ev[1], st));
+        CU(cudaMemcpy(out, ctx->d_grab_stage.p, total, cudaMemcpyDeviceToHost));
+        cudaEventElapsedTime(&ctx->timing.grab_ms, ctx->ev[0], ctx->ev[1]);
+        return R433B_OK;
+    }
+    struct Group {
+        uint8_t const *src;
+        unsigned flip;
+        std::vector<GrabSeg> segs; // staging positions relative to the group's region
+        uint64_t bytes = 0, at = 0;
+    };
+    std::vector<Group> groups;
+    std::vector<std::pair<uint32_t, uint64_t>> place(segs.size()); // segment -> group, its staging position
+    for (size_t i = 0; i < segs.size(); ++i) {
+        uint32_t const s = seg_stream[i];
+        uint8_t const *src = s == UINT32_MAX ? nullptr : ctx->mixed[s].src;
+        unsigned const flip = s == UINT32_MAX ? 0u : ctx->mixed[s].flip;
+        size_t g = 0;
+        while (g < groups.size() && !(s == UINT32_MAX || (groups[g].src == src && groups[g].flip == flip))) ++g;
+        if (g == groups.size()) groups.push_back(Group{src, flip, {}});
+        GrabSeg q = segs[i];
+        q.dst = groups[g].bytes;
+        groups[g].segs.push_back(q);
+        groups[g].bytes += q.len;
+        place[i] = {(uint32_t)g, q.dst};
+    }
+    uint64_t staged = 0;
+    for (Group &g : groups) {
+        g.at = staged;
+        staged += (g.bytes + kGrabSpan - 1) / kGrabSpan * kGrabSpan;
+    }
+    if (int r = dev_reserve(ctx, ctx->d_grab_stage, staged)) return r;
     CU(cudaEventRecord(ctx->ev[0], st));
-    if (int r = grab_launch(ctx, segs, total, (uint8_t const *)prior, ctx->d_grab_stage.p)) return r;
+    for (Group const &g : groups)
+        if (int r = grab_launch(ctx, g.segs, g.bytes, g.src, g.flip, (uint8_t const *)prior, (uint8_t *)ctx->d_grab_stage.p + g.at))
+            return r;
     CU(cudaEventRecord(ctx->ev[1], st));
-    CU(cudaMemcpy(out, ctx->d_grab_stage.p, total, cudaMemcpyDeviceToHost));
+    std::vector<uint8_t> host(staged);
+    CU(cudaMemcpy(host.data(), ctx->d_grab_stage.p, staged, cudaMemcpyDeviceToHost));
     cudaEventElapsedTime(&ctx->timing.grab_ms, ctx->ev[0], ctx->ev[1]);
+    for (size_t i = 0; i < segs.size(); ++i)
+        memcpy(out + segs[i].dst, host.data() + groups[place[i].first].at + place[i].second, segs[i].len);
     return R433B_OK;
 }
 
@@ -2360,7 +2730,7 @@ int chain_grab_append_launch(r433b_ctx *ctx, r433b_chain *ch)
         CU(cudaEventRecord(ctx->ev[0], st));
         if (pre) {
             if (int r = dev_reserve(ctx, ch->d_pre, (pre + kGrabSpan - 1) / kGrabSpan * kGrabSpan)) return r;
-            if (int r = grab_launch(ctx, segs, pre, nullptr, ch->d_pre.p)) return r;
+            if (int r = grab_launch(ctx, segs, pre, ctx->grab_src, ctx->grab_flip, nullptr, ch->d_pre.p)) return r;
         }
         if (max_words) {
             CU(cudaMemcpyAsync(ch->d_ring_slots.p, slots.data(), n * sizeof(GrabRingSlot), cudaMemcpyHostToDevice, st));
@@ -2409,7 +2779,7 @@ void grab_replay(r433b_ctx *ctx, r433b_results const *res, int mode, uint32_t s,
         bool flush, GrabFrame &f, uint32_t &counter, uint32_t &k)
 {
     uint32_t const S = R433B_GRAB_RING;
-    uint32_t const SS = ctx->batch.sample_format, B = ctx->batch.block_bytes;
+    uint32_t const SS = stream_format(ctx, s).SS, B = ctx->batch.block_bytes;
     r433b_package const *pk = res->packages;
     uint32_t const n_pk = res->n_packages;
     uint64_t const L = ctx->lengths[s];
@@ -2555,11 +2925,12 @@ int r433b_grab_copy(r433b_ctx *ctx, r433b_results const *res, uint32_t first, ui
         CU(cudaSetDevice(ctx->device));
         uint64_t dst = 0;
         std::vector<GrabSeg> segs;
+        std::vector<uint32_t> seg_stream;
         for (uint32_t i = first; i < first + count; ++i) {
             r433b_grab const &g = ctx->grabs[i];
             auto segments = [&](int64_t a, int64_t b) {
                 if (ctx->chained) chain_grab_segments(ctx, ctx->chain_last, g.stream, a, b, dst, segs);
-                else grab_segments(ctx, a, b, dst, segs);
+                else grab_segments(ctx, a, b, dst, segs, seg_stream);
             };
             int64_t const lo = g.run_end - (int64_t)g.bytes, hi = g.run_end;
             // positions older than the ring holds read its newest bytes at the same slots (one wrap at most: bytes <= ring)
@@ -2571,7 +2942,7 @@ int r433b_grab_copy(r433b_ctx *ctx, r433b_results const *res, uint32_t first, ui
                 segments(lo, hi);
         }
         if (dst > cap || (dst && !out)) return fail(ctx, R433B_EINVAL, "output buffer smaller than the grabs' bytes");
-        return grab_gather(ctx, segs, dst, out);
+        return grab_gather(ctx, segs, seg_stream, dst, out);
     } catch (std::exception const &) { // allocation failures of the host vectors
         return fail(ctx, R433B_ENOMEM, "r433b_grab_copy: out of host memory");
     }
@@ -2588,9 +2959,10 @@ int r433b_grab_tail(r433b_ctx *ctx, r433b_results const *res, uint8_t *tail, uin
         int64_t const begin = std::max<int64_t>(0, end - (int64_t)R433B_GRAB_RING);
         uint64_t dst = 0;
         std::vector<GrabSeg> segs;
-        grab_segments(ctx, begin, end, dst, segs);
+        std::vector<uint32_t> seg_stream;
+        grab_segments(ctx, begin, end, dst, segs, seg_stream);
         *pushed = (uint64_t)end;
-        return grab_gather(ctx, segs, dst, tail);
+        return grab_gather(ctx, segs, seg_stream, dst, tail);
     } catch (std::exception const &) { // allocation failures of the host vectors
         return fail(ctx, R433B_ENOMEM, "r433b_grab_tail: out of host memory");
     }

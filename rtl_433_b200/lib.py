@@ -33,7 +33,7 @@ EXPORTS = ["r433b_create", "r433b_destroy", "r433b_last_error", "r433b_set_level
            "r433b_dispatch_r_devices_parallel", "r433b_analyze", "r433b_analysis_get", "r433b_analysis_text",
            "r433b_analysis_events", "r433b_submit", "r433b_wait", "r433b_grab_plan", "r433b_grab_copy", "r433b_grab_tail",
            "r433b_chain_create", "r433b_chain_destroy", "r433b_process_chained", "r433b_chain_base",
-           "r433b_chain_grab", "r433b_set_split", "r433b_chain_split"]
+           "r433b_chain_grab", "r433b_set_split", "r433b_chain_split", "r433b_process_mixed"]
 
 
 def build(force=False, verbose=False):
@@ -115,7 +115,12 @@ class Timing(C.Structure):
                 ("front_repairs", C.c_uint32), ("idle_skipped", C.c_uint32), ("idle_rewalks", C.c_uint32),
                 ("grab_ms", C.c_float), ("chain_folds", C.c_uint32), ("chain_fm_rebuilds", C.c_uint32),
                 ("grab_ring_ms", C.c_float), ("split_segments", C.c_uint32), ("split_rewalks", C.c_uint32),
-                ("split_rounds", C.c_uint32), ("split_merge_ms", C.c_float)]
+                ("split_rounds", C.c_uint32), ("split_merge_ms", C.c_float), ("mixed_classes", C.c_uint32),
+                ("mixed_order_ms", C.c_float)]
+
+
+class StreamFormat(C.Structure):
+    _fields_ = [("sample_format", C.c_uint32), ("samp_rate", C.c_uint32), ("center_frequency", C.c_uint32)]
 
 
 SPLIT_AUTO = 0xFFFFFFFF  # r433b_set_split: segment size chosen from the batch's shape
@@ -172,6 +177,7 @@ def load():
     L.r433b_set_devices.argtypes = [C.c_void_p, C.POINTER(Device), C.c_uint32]
     L.r433b_set_r_devices.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
     L.r433b_process.argtypes = [C.c_void_p, C.POINTER(Batch)]
+    L.r433b_process_mixed.argtypes = [C.c_void_p, C.POINTER(Batch), C.POINTER(StreamFormat)]
     L.r433b_chain_create.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_void_p)]
     L.r433b_chain_destroy.argtypes = [C.c_void_p]
     L.r433b_process_chained.argtypes = [C.c_void_p, C.POINTER(Batch), C.c_void_p, C.c_void_p]
@@ -496,6 +502,28 @@ class Context:
                 raise R433Error("corrupt analyzer event stream")
             at += used.value
         return a, g, buf.value.decode(), bbs
+
+    def process_mixed(self, data, offsets, formats, rates, freqs, lengths=None, fpdm_mode=FPDM_AUTO, data_on_device=False,
+                      block_bytes=0):
+        """A batch whose stream i has its own sample format, rate and centre frequency (formats[i], rates[i], freqs[i];
+        include/r433b.h: r433b_process_mixed).  `data`: host numpy array or an int device pointer."""
+        offs = np.ascontiguousarray(offsets, dtype=np.uint64)
+        n = len(offs) - 1
+        if not (len(formats) == len(rates) == len(freqs) == n):
+            raise ValueError("one format, rate and centre frequency per stream")
+        if isinstance(data, int):
+            ptr = data
+        else:
+            data = np.ascontiguousarray(data)
+            ptr = data.ctypes.data
+        lens = None if lengths is None else np.ascontiguousarray(lengths, dtype=np.uint64)
+        fmt = (StreamFormat * max(1, n))()
+        for i in range(n):
+            fmt[i] = StreamFormat(int(formats[i]), int(rates[i]), int(freqs[i]))
+        b = Batch(ptr, offs.ctypes.data_as(C.POINTER(C.c_uint64)), n, 0, 0, 0, fpdm_mode, block_bytes, int(data_on_device), 0,
+                  None if lens is None else lens.ctypes.data_as(C.POINTER(C.c_uint64)))
+        self._keep = (data, offs, lens)
+        self._check(self.L.r433b_process_mixed(self.h, C.byref(b), fmt))
 
     def submit(self, data, offsets, sample_format, samp_rate=250000, center_frequency=433920000, fpdm_mode=FPDM_AUTO,
                block_bytes=0, data_on_device=False, lengths=None):
