@@ -210,9 +210,9 @@ int r433b_process(r433b_ctx *ctx, r433b_batch const *batch);
    - Per stream: the rate is not 0; the offset is a multiple of 16 bytes (32 for cf32).  Without lengths the offsets
      ascend and stream i fills its gap; with lengths, stream i is [offsets[i], offsets[i] + lengths[i]), which must end by
      offsets[n_streams], and the offsets need not ascend.
-   - want_stages returns R433B_EINVAL.  There is no chained (r433b_process_chained) and no asynchronous (r433b_submit)
-     form.  A mixed batch runs unsplit whatever r433b_set_split says, and host input goes to the device in one copy,
-     without time slices (r433b_set_pipeline).
+   - want_stages returns R433B_EINVAL.  There is no asynchronous (r433b_submit) form; the chained form is
+     r433b_process_mixed_chained() below.  A mixed batch runs unsplit whatever r433b_set_split says, and host input
+     goes to the device in one copy, without time slices (r433b_set_pipeline).
    - Streams that one detector launch can walk together (the same sample size after load-time conversion, cs8 flip,
      rate and resolved FPDM) form a class.  Each class is one launch of k_front and k_detect; the launches run
      side by side on a small pool of CUDA streams.  r433b_timing: front_ms is the wall time from the first launch to
@@ -298,6 +298,29 @@ int r433b_chain_grab(r433b_chain *chain, int mode);
      overflow reruns the schedule from the state the chain carried.
    - Memory on the device: that of r433b_set_split for the batch's segments, in the context. */
 int r433b_chain_split(r433b_chain *chain, uint32_t segment_blocks, uint32_t warmup_blocks);
+/* Mixed batches on a chain: several receivers on different bands, one slot each, or a corpus of mixed formats too large
+   for the device.  Batch stream i is the next chunk of slot i's file, described by fmt[i]; for every slot the results
+   are those of its files processed uncut and alone (the chain rule above, with the per-stream formats of
+   r433b_process_mixed()): every r433b_package field including seq, offset, end_pos and block, the widths, pairs,
+   events, analyzer text, pulse_data_t and sample_file_pos.
+   - The batch's arguments are those of r433b_process_mixed(), the chain's those of r433b_process_chained(): n_streams
+     equals the chain's, the chain belongs to this context, and a chunk that is not its file's last is whole blocks of
+     that slot's own input (2 x block_bytes for cf32).  want_stages and a null fmt return R433B_EINVAL.
+   - A slot's sample format, rate, centre frequency and resolved FPDM may change only at that slot's file start.
+     block_bytes, the levels, the FM low-pass and whether FM is on are shared by the whole chain and may not change
+     while any slot is inside a file.  Both return R433B_ESTATE.
+   - A chain whose open files were begun by this call refuses r433b_process_chained(), and one whose open files were
+     begun by r433b_process_chained() refuses this call, both with R433B_ESTATE.  While every slot is at a file start,
+     either may follow.
+   - A refused call leaves the context and the chain as they were.  A chain's state is written only once the whole
+     batch has succeeded, so an arena overflow reruns from the state the chain carried.
+   - It runs unsplit, also on a chain that opted into r433b_chain_split (r433b_timing.split_segments is 0).  There is
+     no asynchronous form, and host input goes to the device in one copy per call.
+   - The grabber works as on any chain (r433b_chain_grab, while every slot is at a file start): each slot is its own
+     run across its files, whatever their formats, and its grabs equal those of one r433b_process_mixed() batch
+     holding that slot's files in order. */
+int r433b_process_mixed_chained(r433b_ctx *ctx, r433b_batch const *batch, r433b_stream_format const *fmt,
+                                r433b_chain *chain, uint8_t const *last);
 
 /* Copy the compact results to host memory owned by the context. */
 int r433b_fetch(r433b_ctx *ctx, r433b_results *out);

@@ -165,15 +165,24 @@ struct r433b_ctx {
     DevBuf d_mx_tab, d_mx_pkgs;
 };
 
-// What must not change while a chain has an open file: everything the carried state depends on
+// What the carried state depends on: per slot its format, which must not change inside one of its files ...
+struct SlotFormat {
+    uint32_t sample_format, samp_rate, center_frequency, fpdm;
+    bool operator==(SlotFormat const &o) const
+    {
+        return sample_format == o.sample_format && samp_rate == o.samp_rate && center_frequency == o.center_frequency
+                && fpdm == o.fpdm;
+    }
+};
+
+// ... and what the whole chain shares, which must not change while any of its slots has an open file
 struct ChainSettings {
-    uint32_t sample_format, samp_rate, center_frequency, fpdm, block_bytes;
+    uint32_t block_bytes;
     int use_mag, enable_fm;
     float level_limit, min_level, min_snr, fm_low_pass;
     bool operator==(ChainSettings const &o) const
     {
-        return sample_format == o.sample_format && samp_rate == o.samp_rate && center_frequency == o.center_frequency
-                && fpdm == o.fpdm && block_bytes == o.block_bytes && use_mag == o.use_mag && enable_fm == o.enable_fm
+        return block_bytes == o.block_bytes && use_mag == o.use_mag && enable_fm == o.enable_fm
                 && level_limit == o.level_limit && min_level == o.min_level && min_snr == o.min_snr
                 && fm_low_pass == o.fm_low_pass;
     }
@@ -189,6 +198,8 @@ struct r433b_chain {
     std::vector<uint64_t> next;    // ... whose next chunk starts at this absolute sample
     std::vector<uint64_t> base;    // first sample of slot i's chunk in the last chained batch
     ChainSettings settings{};
+    std::vector<SlotFormat> fmt;   // per slot, of the last chained batch
+    bool mixed = false;            // the last chained batch was r433b_process_mixed_chained(): so are the open files
     // segmented replay of this chain's batches (r433b_chain_split): segment / warm-up blocks, 0: off
     uint32_t split_blocks = 0, split_warmup = 1;
     // signal grabber (r433b_chain_grab): each slot is its own run with a kGrabRingBytes ring on the device
@@ -599,9 +610,42 @@ struct Shape {
     bool cf32;       // cf32 becomes cs16 on the device before anything else (src/rtl_433.c:1811-1825): from there on
     unsigned in_div; // offsets, lengths and byte counts are those of the cs16 stream (the input's / in_div)
     int SS;          // bytes per IQ sample; cs8 is cu8 after the load-time +128
+    SlotFormat fmt;  // every stream's
     ChainSettings settings;
     uint64_t total_bytes, used_bytes, max_samples; // the last two of the lengths in use (adopt_batch)
 };
+
+// A chained batch's chain arguments: slot i's format fmt[i] and input bytes in_bytes[i]; `mixed`: the batch is
+// r433b_process_mixed_chained()'s.  Changes nothing in the context but the error string.
+int check_chain(r433b_ctx *ctx, r433b_batch const *b, r433b_chain const *ch, uint8_t const *last,
+        ChainSettings const &settings, bool mixed, std::vector<SlotFormat> const &fmt, std::vector<uint64_t> const &in_bytes)
+{
+    std::string const who = mixed ? "r433b_process_mixed_chained: " : "r433b_process_chained: ";
+    auto refuse = [&](int code, char const *what) { return fail(ctx, code, (who + what).c_str()); };
+    if (ch->ctx != ctx || !last) return refuse(R433B_EINVAL, "chain of another context, or no last[]");
+    if (b->n_streams != ch->n) return refuse(R433B_EINVAL, "n_streams differs from the chain's");
+    if (ch->grab_failed) return refuse(R433B_ESTATE, "a batch of this grabbing chain failed while appending to its rings");
+    if (ch->grab_pending)
+        return refuse(R433B_ESTATE, "the grabbing chain's last batch was not planned (r433b_grab_plan): its frames would "
+                                    "be lost");
+    bool const open = std::find(ch->open.begin(), ch->open.end(), 1) != ch->open.end();
+    if (open && ch->mixed != mixed)
+        return refuse(R433B_ESTATE, mixed ? "the chain's open files were begun by r433b_process_chained"
+                                          : "the chain's open files were begun by r433b_process_mixed_chained");
+    bool changed = open && !(settings == ch->settings);
+    for (uint32_t i = 0; i < b->n_streams && !changed; ++i) changed = ch->open[i] && !(fmt[i] == ch->fmt[i]);
+    if (changed)
+        return refuse(R433B_ESTATE, "format, rate, frequency, block size, levels or FM settings changed while a file of "
+                                    "the chain is open");
+    // a chunk that the file goes on behind is whole blocks: the next one starts on a block boundary
+    for (uint32_t i = 0; i < b->n_streams; ++i) {
+        uint64_t const in_div = fmt[i].sample_format == R433B_FMT_CF32 ? 2 : 1;
+        if (!last[i] && in_bytes[i] % ((uint64_t)settings.block_bytes * in_div))
+            return refuse(R433B_EINVAL, "a chunk that is not its file's last must be whole blocks (block_bytes, 2 x "
+                                        "block_bytes of cf32 input)");
+    }
+    return R433B_OK;
+}
 
 // The batch's arguments, and the chain's if it has one.  Changes nothing in the context but the error string.
 int check_batch(r433b_ctx *ctx, r433b_batch const *b, r433b_chain const *ch, uint8_t const *last, Shape &s)
@@ -626,29 +670,13 @@ int check_batch(r433b_ctx *ctx, r433b_batch const *b, r433b_chain const *ch, uin
         if (d.modulation >= 16) enable_fm = 1;
     // src/rtl_433.c:1094-1102 and :1515-1522
     unsigned const fpdm = b->fpdm_mode == R433B_FPDM_AUTO ? (b->center_frequency > 800000000u ? 1u : 0u) : b->fpdm_mode;
-    s.settings = ChainSettings{b->sample_format, b->samp_rate, b->center_frequency, fpdm, block_bytes, ctx->use_mag, enable_fm,
-                               ctx->level_limit, ctx->min_level, ctx->min_snr, ctx->fm_low_pass};
-    if (ch) {
-        if (ch->ctx != ctx || !last) return fail(ctx, R433B_EINVAL, "r433b_process_chained: chain of another context, or no last[]");
-        if (b->n_streams != ch->n) return fail(ctx, R433B_EINVAL, "r433b_process_chained: n_streams differs from the chain's");
-        if (ch->grab_failed)
-            return fail(ctx, R433B_ESTATE, "r433b_process_chained: a batch of this grabbing chain failed while "
-                                           "appending to its rings");
-        if (ch->grab_pending)
-            return fail(ctx, R433B_ESTATE, "r433b_process_chained: the grabbing chain's last batch was not planned "
-                                           "(r433b_grab_plan): its frames would be lost");
-        if (std::find(ch->open.begin(), ch->open.end(), 1) != ch->open.end() && !(s.settings == ch->settings))
-            return fail(ctx, R433B_ESTATE, "r433b_process_chained: format, rate, frequency, block size, levels or FM "
-                                           "settings changed while a file of the chain is open");
-        // a chunk that the file goes on behind is whole blocks: the next one starts on a block boundary
-        for (uint32_t i = 0; i < b->n_streams; ++i) {
-            uint64_t const in_bytes = b->lengths ? b->lengths[i] : b->offsets[i + 1] - b->offsets[i];
-            if (!last[i] && in_bytes % ((uint64_t)block_bytes * s.in_div))
-                return fail(ctx, R433B_EINVAL, "r433b_process_chained: a chunk that is not its file's last must be whole "
-                                               "blocks (block_bytes, 2 x block_bytes of cf32 input)");
-        }
-    }
-    return R433B_OK;
+    s.fmt = SlotFormat{b->sample_format, b->samp_rate, b->center_frequency, fpdm};
+    s.settings = ChainSettings{block_bytes, ctx->use_mag, enable_fm, ctx->level_limit, ctx->min_level, ctx->min_snr,
+                               ctx->fm_low_pass};
+    if (!ch) return R433B_OK;
+    std::vector<uint64_t> in_bytes(b->n_streams);
+    for (uint32_t i = 0; i < b->n_streams; ++i) in_bytes[i] = b->lengths ? b->lengths[i] : b->offsets[i + 1] - b->offsets[i];
+    return check_chain(ctx, b, ch, last, s.settings, false, std::vector<SlotFormat>(b->n_streams, s.fmt), in_bytes);
 }
 
 // The batch becomes the context's last one (the host replay reads it), and the results of the one before are gone
@@ -738,7 +766,7 @@ int prepare_detect(r433b_ctx *ctx, r433b_batch const *b, Shape const &s, DetectP
     dp.use_mag = ctx->use_mag;
     dp.flip = dp_flip_of(b->sample_format);
     dp.enable_fm = s.settings.enable_fm;
-    dp.fpdm = (int)s.settings.fpdm;
+    dp.fpdm = (int)s.fmt.fpdm;
     dp.rate = b->samp_rate;
     dp.block_samples = s.settings.block_bytes / SS;
     dp.lv = ctx->lv;
@@ -770,41 +798,56 @@ int bind_detector_arenas(r433b_ctx *ctx, DetectParams &dp)
 }
 
 // A chained batch: the chain's state and pulse trains, which slots continue a file, which files end, where each chunk
-// lies in its file (chain_base).  The state is copied first, so that a run that has to be repeated starts from it again.
-int chain_begin(r433b_ctx *ctx, r433b_chain *ch, uint8_t const *last, DetectParams &dp)
+// lies in its file (chain_base, in slot order).  The state is copied first, so that a run that has to be repeated
+// starts from it again.  A mixed batch (`order`: the slot of internal stream j) walks its streams in internal order: the
+// flags and bases go to the device permuted, and the walk uses the copies, into which the caller gathers the state
+// (k_split_chain_in) at every attempt; the chain's own state is written only once the batch has succeeded.
+int chain_begin(r433b_ctx *ctx, r433b_chain *ch, uint8_t const *last, DetectParams &dp,
+        std::vector<uint32_t> const *order = nullptr)
 {
     if (!ch) return R433B_OK;
     size_t const n = ch->n;
     std::vector<uint8_t> flags(2 * n);
+    std::vector<uint64_t> base(n);
     ctx->chain_base.resize(n);
-    for (size_t i = 0; i < n; ++i) {
-        flags[i] = ch->open[i];
-        flags[n + i] = last[i] ? 1 : 0;
-        ctx->chain_base[i] = ch->open[i] ? ch->next[i] : 0;
+    for (size_t i = 0; i < n; ++i) ctx->chain_base[i] = ch->open[i] ? ch->next[i] : 0;
+    for (size_t j = 0; j < n; ++j) {
+        size_t const i = order ? (*order)[j] : j;
+        flags[j] = ch->open[i];
+        flags[n + j] = last[i] ? 1 : 0;
+        base[j] = ctx->chain_base[i];
     }
     CU(cudaMemcpy(ch->d_flags.p, flags.data(), 2 * n, cudaMemcpyHostToDevice));
-    CU(cudaMemcpy(ch->d_base.p, ctx->chain_base.data(), n * sizeof(uint64_t), cudaMemcpyHostToDevice));
-    CU(cudaMemcpyAsync(ch->d_state_copy.p, ch->d_state.p, n * sizeof(StreamState), cudaMemcpyDeviceToDevice, 0));
-    CU(cudaMemcpyAsync(ch->d_train_copy.p, ch->d_train.p, n * kTrainInts * sizeof(int), cudaMemcpyDeviceToDevice, 0));
-    dp.state = (StreamState *)ch->d_state.p;
+    CU(cudaMemcpy(ch->d_base.p, base.data(), n * sizeof(uint64_t), cudaMemcpyHostToDevice));
     dp.cont = (unsigned char const *)ch->d_flags.p;
     dp.last = (unsigned char const *)ch->d_flags.p + n;
     dp.base = (unsigned long long const *)ch->d_base.p;
+    if (order) {
+        dp.state = (StreamState *)ch->d_state_copy.p;
+        dp.train_scratch = (int *)ch->d_train_copy.p;
+        return R433B_OK;
+    }
+    CU(cudaMemcpyAsync(ch->d_state_copy.p, ch->d_state.p, n * sizeof(StreamState), cudaMemcpyDeviceToDevice, 0));
+    CU(cudaMemcpyAsync(ch->d_train_copy.p, ch->d_train.p, n * kTrainInts * sizeof(int), cudaMemcpyDeviceToDevice, 0));
+    dp.state = (StreamState *)ch->d_state.p;
     dp.train_scratch = (int *)ch->d_train.p;
     return R433B_OK;
 }
 
 // The batch has succeeded: the chain moves on, and a grabbing chain appends the chunks to its rings (once, also after a
-// run that was repeated)
-int chain_finish(r433b_ctx *ctx, r433b_chain *ch, uint8_t const *last, Shape const &s)
+// run that was repeated).  fmt: every slot's format.
+int chain_finish(r433b_ctx *ctx, r433b_chain *ch, uint8_t const *last, ChainSettings const &settings,
+        std::vector<SlotFormat> const &fmt, bool mixed)
 {
     if (!ch) return R433B_OK;
     for (uint32_t i = 0; i < ch->n; ++i) {
         ch->open[i] = last[i] ? 0 : 1;
-        ch->next[i] = last[i] ? 0 : ctx->chain_base[i] + ctx->lengths[i] / s.SS;
+        ch->next[i] = last[i] ? 0 : ctx->chain_base[i] + ctx->lengths[i] / stream_format(ctx, i).SS;
     }
     ch->base = ctx->chain_base;
-    ch->settings = s.settings;
+    ch->settings = settings;
+    ch->fmt = fmt;
+    ch->mixed = mixed;
     ctx->chained = true;
     ctx->chain_last = ch;
     if (!ch->grab_mode) return R433B_OK;
@@ -1459,7 +1502,7 @@ int process_iq(r433b_ctx *ctx, r433b_batch const *b, r433b_chain *ch, uint8_t co
     ctx->timing.d2h_ms = 0; // r433b_fetch()'s, or overlapped
     ctx->n_samples = s.used_bytes / s.SS;
     ctx->processed = true;
-    return chain_finish(ctx, ch, last, s);
+    return chain_finish(ctx, ch, last, s.settings, std::vector<SlotFormat>(b->n_streams, s.fmt), false);
 }
 
 // ---- mixed batches (r433b_process_mixed, DESIGN §7d) -----------------------------------------------------------------
@@ -1477,8 +1520,11 @@ struct MixedClass {
 };
 
 // rtl_433 -r f1 -r f2 ... on a batch of files of their own formats: one k_front + k_detect launch per class on the
-// CUDA stream pool, k_mixed_order, then the slicers over one package range per rate.
-int process_mixed(r433b_ctx *ctx, r433b_batch const *b, r433b_stream_format const *fmt)
+// CUDA stream pool, k_mixed_order, then the slicers over one package range per rate.  With a chain, stream i is the
+// next chunk of slot i's file: the slots' state is gathered into internal order in front of every attempt and
+// scattered back once the batch has succeeded (DESIGN §7d).
+int process_mixed(r433b_ctx *ctx, r433b_batch const *b, r433b_stream_format const *fmt, r433b_chain *ch,
+        uint8_t const *last)
 {
     if (!ctx || !b || !b->offsets || (b->n_streams && (!b->data || !fmt))) return fail(ctx, R433B_EINVAL, "null argument");
     if (b->sample_format || b->samp_rate || b->center_frequency)
@@ -1494,7 +1540,7 @@ int process_mixed(r433b_ctx *ctx, r433b_batch const *b, r433b_stream_format cons
         if (d.modulation >= 16) enable_fm = 1;
     // per stream: checks, its class key, its bytes after conversion (cf32 -> cs16, in the conversion region)
     std::vector<MixedClass> key(n);
-    std::vector<uint64_t> len(n), conv(n, UINT64_MAX);
+    std::vector<uint64_t> len(n), in_lens(n), conv(n, UINT64_MAX);
     uint64_t conv_bytes = 0;
     for (uint32_t i = 0; i < n; ++i) {
         uint32_t const f = fmt[i].sample_format;
@@ -1509,6 +1555,7 @@ int process_mixed(r433b_ctx *ctx, r433b_batch const *b, r433b_stream_format cons
         if (!b->lengths && b->offsets[i + 1] < b->offsets[i]) return fail(ctx, R433B_EINVAL, "offsets not ascending");
         if (b->offsets[i] > total || in_len > total - b->offsets[i])
             return fail(ctx, R433B_EINVAL, "a stream ends behind offsets[n_streams]");
+        in_lens[i] = in_len;
         len[i] = in_div == 2 ? in_len / 8 * 4 : in_len; // whole IQ pairs of floats -> cs16 bytes
         if (in_div == 2) {
             conv[i] = conv_bytes;
@@ -1517,6 +1564,12 @@ int process_mixed(r433b_ctx *ctx, r433b_batch const *b, r433b_stream_format cons
         uint32_t const fpdm = b->fpdm_mode == R433B_FPDM_AUTO ? (fmt[i].center_frequency > 800000000u ? 1u : 0u) : b->fpdm_mode;
         key[i] = MixedClass{fmt[i].samp_rate, SS, dp_flip_of(f), fpdm, in_div == 2 && b->data_on_device ? 1u : 0u, 0, 0, 0};
     }
+    ChainSettings const settings{block_bytes, ctx->use_mag, enable_fm, ctx->level_limit, ctx->min_level, ctx->min_snr,
+                                 ctx->fm_low_pass};
+    std::vector<SlotFormat> slots(n);
+    for (uint32_t i = 0; i < n; ++i) slots[i] = SlotFormat{fmt[i].sample_format, fmt[i].samp_rate, fmt[i].center_frequency, key[i].fpdm};
+    if (ch)
+        if (int r = check_chain(ctx, b, ch, last, settings, true, slots, in_lens)) return r;
     CU(cudaSetDevice(ctx->device));
 
     // the batch becomes the context's last one
@@ -1599,11 +1652,21 @@ int process_mixed(r433b_ctx *ctx, r433b_batch const *b, r433b_stream_format cons
     if (int r = dev_reserve(ctx, ctx->d_am, am_samples * sizeof(int16_t) + 16)) return r;
     if (int r = dev_reserve(ctx, ctx->d_chunks, am_samples / kChunk * sizeof(ChunkInfo) + 16)) return r;
     if (int r = dev_reserve(ctx, ctx->d_tiles, am_samples / kTile * sizeof(TileInfo) + 16)) return r;
-    if (int r = dev_reserve(ctx, ctx->d_mx_tab, (2 * n + 1) * sizeof(uint32_t))) return r;
+    // d_mx_tab: the caller's index of every internal stream, k_mixed_order's bases (n + 1); chained: per internal stream
+    // the seq it starts from, per slot its internal stream and whether it continues a file (bytes)
+    if (int r = dev_reserve(ctx, ctx->d_mx_tab, (4 * n + 1) * sizeof(uint32_t) + n)) return r;
     CU(cudaMemcpy(ctx->d_offsets.p, off, (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice));
     if (n) CU(cudaMemcpy(ctx->d_lengths.p, lens, n * sizeof(uint64_t), cudaMemcpyHostToDevice));
     CU(cudaMemcpy(ctx->d_amoff.p, amoff, (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice));
     if (n) CU(cudaMemcpy(ctx->d_mx_tab.p, caller_of.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    unsigned *const start_seq = (unsigned *)ctx->d_mx_tab.p + 2 * n + 1, *const internal_of = start_seq + n;
+    unsigned char *const slot_cont = (unsigned char *)(internal_of + n);
+    if (ch && n) {
+        std::vector<uint32_t> in_of(n);
+        for (uint32_t j = 0; j < n; ++j) in_of[order[j]] = j;
+        CU(cudaMemcpy(internal_of, in_of.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(slot_cont, ch->open.data(), n, cudaMemcpyHostToDevice));
+    }
     if (int r = upload_slicer_tables(ctx, rates, 0)) return r;
     ctx->pkg_cap = std::max<size_t>(ctx->pkg_cap, ctx->min_caps[0] ? ctx->min_caps[0] : (size_t)n * 16 + 1024);
     ctx->pool_cap = std::max<size_t>(ctx->pool_cap, ctx->min_caps[1] ? ctx->min_caps[1] : ctx->pkg_cap * 128);
@@ -1627,6 +1690,7 @@ int process_mixed(r433b_ctx *ctx, r433b_batch const *b, r433b_stream_format cons
     dp.am = (int16_t *)ctx->d_am.p;
     dp.chunks = (ChunkInfo const *)ctx->d_chunks.p;
     dp.tile_info = (TileInfo const *)ctx->d_tiles.p;
+    if (int r = chain_begin(ctx, ch, last, dp, &order)) return r;
     size_t const n_launch = classes.size();
     while (ctx->ev_mx.size() < 2 * n_launch) {
         cudaEvent_t e;
@@ -1652,6 +1716,13 @@ int process_mixed(r433b_ctx *ctx, r433b_batch const *b, r433b_stream_format cons
     for (int attempt = 0;; ++attempt) {
         if (int r = bind_detector_arenas(ctx, dp)) return r;
         CU(cudaMemsetAsync(ctx->d_counters.p, 0, 64, st));
+        if (ch) { // from the chain, which only the scatter below writes: also where an overflow reruns from
+            CU(cudaMemsetAsync(start_seq, 0, n * sizeof(unsigned), st));
+            R4_LAUNCH(k_split_chain_in, (n + kSplitWarps - 1) / kSplitWarps, kSplitWarps * 32, 0, st,
+                      (StreamState const *)ch->d_state.p, (int const *)ch->d_train.p, (unsigned char const *)slot_cont,
+                      (unsigned const *)internal_of, n, (StreamState *)dp.state, dp.train_scratch, start_seq);
+            CU(cudaGetLastError());
+        }
         CU(cudaEventRecord(ctx->ev[4], st)); // the classes start here
         for (size_t c = 0; c < n_launch; ++c) {
             MixedClass const &k = classes[c];
@@ -1698,6 +1769,7 @@ int process_mixed(r433b_ctx *ctx, r433b_batch const *b, r433b_stream_format cons
         mo.n_streams = n;
         mo.caller = (unsigned const *)ctx->d_mx_tab.p;
         mo.base = (unsigned *)ctx->d_mx_tab.p + n;
+        mo.start_seq = ch ? start_seq : nullptr;
         unsigned const grid = (unsigned)std::min<uint64_t>((uint64_t)ctx->n_sms * 4, (ctx->n_pkgs + kMixedThreads - 1) / kMixedThreads);
         CU(cudaMemsetAsync(mo.base, 0, (n + 1) * sizeof(unsigned), st));
         R4_LAUNCH(k_mixed_order, grid, kMixedThreads, 0, st, mo, 0);
@@ -1715,6 +1787,12 @@ int process_mixed(r433b_ctx *ctx, r433b_batch const *b, r433b_stream_format cons
         ranges[g].pkg_end = base[slot_first[g + 1]];
     }
     if (int r = slice_ranges(ctx, ranges, ctx->n_pkgs, ctx->pool_used, st)) return r;
+    if (ch && n) { // the batch has succeeded: the walks' end states back to their slots
+        R4_LAUNCH(k_split_scatter, (n + kSplitWarps - 1) / kSplitWarps, kSplitWarps * 32, 0, st,
+                  (StreamState const *)dp.state, (int const *)dp.train_scratch, (unsigned const *)ctx->d_mx_tab.p, n,
+                  (StreamState *)ch->d_state.p, (int *)ch->d_train.p);
+        CU(cudaGetLastError());
+    }
 
     auto ms = [](cudaEvent_t a, cudaEvent_t e) { float t = 0; cudaEventElapsedTime(&t, a, e); return t; };
     float front_end = 0, detect_begin = 0, detect_end = 0;
@@ -1735,15 +1813,20 @@ int process_mixed(r433b_ctx *ctx, r433b_batch const *b, r433b_stream_format cons
     ctx->timing.front_repairs = cnt.front_repairs;
     ctx->timing.idle_skipped = cnt.idle_skipped;
     ctx->timing.idle_rewalks = cnt.idle_rewalks;
+    ctx->timing.chain_folds = cnt.chain_folds;
+    ctx->timing.chain_fm_rebuilds = cnt.chain_fm_rebuilds;
     ctx->n_samples = n_samples;
     ctx->processed = true;
-    return R433B_OK;
+    return chain_finish(ctx, ch, last, settings, slots, true);
 }
 
 } // namespace
 
 int r433b_process(r433b_ctx *ctx, r433b_batch const *b) { return process_iq(ctx, b, nullptr, nullptr); }
-int r433b_process_mixed(r433b_ctx *ctx, r433b_batch const *b, r433b_stream_format const *fmt) { return process_mixed(ctx, b, fmt); }
+int r433b_process_mixed(r433b_ctx *ctx, r433b_batch const *b, r433b_stream_format const *fmt)
+{
+    return process_mixed(ctx, b, fmt, nullptr, nullptr);
+}
 
 int r433b_chain_create(r433b_ctx *ctx, uint32_t n_streams, r433b_chain **out)
 {
@@ -1757,6 +1840,7 @@ int r433b_chain_create(r433b_ctx *ctx, uint32_t n_streams, r433b_chain **out)
     ch->n = n_streams;
     ch->open.assign(n_streams, 0);
     ch->next.assign(n_streams, 0);
+    ch->fmt.assign(n_streams, SlotFormat{});
     size_t const n = n_streams;
     for (auto [buf, bytes] : {std::pair<DevBuf *, size_t>{&ch->d_state, n * sizeof(StreamState)}, {&ch->d_state_copy, n * sizeof(StreamState)},
                               {&ch->d_train, n * kTrainInts * sizeof(int)}, {&ch->d_train_copy, n * kTrainInts * sizeof(int)},
@@ -1785,6 +1869,14 @@ int r433b_process_chained(r433b_ctx *ctx, r433b_batch const *b, r433b_chain *cha
 {
     if (!chain || !chain->ctx) return fail(ctx, R433B_EINVAL, "r433b_process_chained: no chain, or its context is gone");
     return process_iq(ctx, b, chain, last);
+}
+
+int r433b_process_mixed_chained(r433b_ctx *ctx, r433b_batch const *b, r433b_stream_format const *fmt, r433b_chain *chain,
+        uint8_t const *last)
+{
+    if (!chain || !chain->ctx)
+        return fail(ctx, R433B_EINVAL, "r433b_process_mixed_chained: no chain, or its context is gone");
+    return process_mixed(ctx, b, fmt, chain, last);
 }
 
 int r433b_chain_grab(r433b_chain *chain, int mode)
@@ -2575,9 +2667,9 @@ void grab_segments(r433b_ctx const *ctx, int64_t a, int64_t b, uint64_t &dst, st
 
 // Slot s's run byte range [a, b) on a grabbing chain after its last batch, as segments: negative positions were never
 // written (zero); the ring holds the newest kGrabRingBytes (split at its wrap); older bytes of the chunk come from the
-// batch, older ones before it from the bytes the append overwrote (saved at d_pre).
+// batch, older ones before it from the bytes the append overwrote (saved at d_pre).  seg_stream as in grab_segments.
 void chain_grab_segments(r433b_ctx const *ctx, r433b_chain const *ch, uint32_t s, int64_t a, int64_t b, uint64_t &dst,
-        std::vector<GrabSeg> &segs)
+        std::vector<GrabSeg> &segs, std::vector<uint32_t> &seg_stream)
 {
     int64_t const S = kGrabRingBytes, c0 = (int64_t)ch->run_c0[s], ring_lo = (int64_t)ch->run[s] - S;
     while (a < b) {
@@ -2602,6 +2694,7 @@ void chain_grab_segments(r433b_ctx const *ctx, r433b_chain const *ch, uint32_t s
             g.src = ch->pre_off[s] + (uint64_t)(a - (int64_t)ch->pre_lo[s]);
         }
         g.len = (uint64_t)(e - a);
+        seg_stream.push_back(g.kind == kGrabBatch ? s : UINT32_MAX);
         segs.push_back(g);
         dst += g.len;
         a = e;
@@ -2694,7 +2787,9 @@ static_assert(kGrabRingBytes == R433B_GRAB_RING, "k_grab_ring's ring size");
 
 // After a grabbing chain's batch: save the ring bytes the append overwrites that the batch's frames may still read
 // (k_grab), then append every slot's chunk to its ring (k_grab_ring).  A frame that ends in this batch ends at a block
-// call, so it reads its slot's run from the end of the chunk's first block minus the ring size on.
+// call, so it reads its slot's run from the end of the chunk's first block minus the ring size on.  The slots of a mixed
+// batch read different buffers with different flips: one k_grab_ring per (buffer, flip), in which the other slots
+// append nothing (n = 0 and w0 = 0 give no words, so their warps return at once).
 int chain_grab_append_launch(r433b_ctx *ctx, r433b_chain *ch)
 {
     try {
@@ -2727,20 +2822,41 @@ int chain_grab_append_launch(r433b_ctx *ctx, r433b_chain *ch)
             slots[s].w0 = (unsigned)((c1 - m) % S);
             max_words = std::max<uint64_t>(max_words, std::min<uint64_t>(((c1 - m) % 16 + m + 15) / 16, S / 16));
         }
+        struct Source {
+            uint8_t const *batch;
+            unsigned flip;
+            std::vector<GrabRingSlot> slots;
+            uint64_t max_words;
+        };
+        std::vector<Source> sources;
+        if (ctx->mixed.empty()) {
+            sources.push_back(Source{ctx->grab_src, ctx->grab_flip, slots, max_words});
+        } else {
+            for (uint32_t s = 0; s < n; ++s) {
+                r433b_ctx::MixedStream const &m = ctx->mixed[s];
+                size_t g = 0;
+                while (g < sources.size() && !(sources[g].batch == m.src && sources[g].flip == m.flip)) ++g;
+                if (g == sources.size()) sources.push_back(Source{m.src, m.flip, std::vector<GrabRingSlot>(n), 0});
+                sources[g].slots[s] = slots[s];
+                sources[g].max_words = std::max<uint64_t>(sources[g].max_words, std::min<uint64_t>(
+                        (slots[s].w0 % 16 + slots[s].n + 15) / 16, S / 16));
+            }
+        }
         CU(cudaEventRecord(ctx->ev[0], st));
-        if (pre) {
+        if (pre) { // ring bytes only: no batch buffer is read
             if (int r = dev_reserve(ctx, ch->d_pre, (pre + kGrabSpan - 1) / kGrabSpan * kGrabSpan)) return r;
             if (int r = grab_launch(ctx, segs, pre, ctx->grab_src, ctx->grab_flip, nullptr, ch->d_pre.p)) return r;
         }
-        if (max_words) {
-            CU(cudaMemcpyAsync(ch->d_ring_slots.p, slots.data(), n * sizeof(GrabRingSlot), cudaMemcpyHostToDevice, st));
+        for (Source const &src : sources) {
+            if (!src.max_words) continue;
+            CU(cudaMemcpyAsync(ch->d_ring_slots.p, src.slots.data(), n * sizeof(GrabRingSlot), cudaMemcpyHostToDevice, st));
             GrabRingParams rp{};
-            rp.batch = ctx->grab_src;
+            rp.batch = src.batch;
             rp.rings = (uint8_t *)ch->d_ring.p;
             rp.slots = (GrabRingSlot const *)ch->d_ring_slots.p;
             uint64_t const per_cta = kGrabThreads / 32 * (kGrabSpan / 16);
-            rp.ctas = (unsigned)((max_words + per_cta - 1) / per_cta);
-            rp.flip = ctx->grab_flip;
+            rp.ctas = (unsigned)((src.max_words + per_cta - 1) / per_cta);
+            rp.flip = src.flip;
             R4_LAUNCH(k_grab_ring, n * rp.ctas, kGrabThreads, 0, st, rp);
             CU(cudaGetLastError());
         }
@@ -2881,11 +2997,12 @@ int r433b_grab_plan(r433b_ctx *ctx, r433b_results const *res, int mode, r433b_gr
         ctx->grab_newest.clear();
         uint32_t k = 0;
         if (ch) { // every slot is its own run: its frame and counter carry over from the slot's last batch
-            uint32_t const SS = ctx->batch.sample_format, B = ctx->batch.block_bytes;
+            uint32_t const B = ctx->batch.block_bytes;
             for (uint32_t s = 0; s < n_streams; ++s) {
                 GrabFrame f = ch->frame[s];
                 uint32_t counter = ch->counter[s];
-                grab_replay(ctx, res, mode, s, ch->run_c0[s], ctx->chain_base[s] * SS / B, ch->ended[s], f, counter, k);
+                uint64_t const blk0 = ctx->chain_base[s] * stream_format(ctx, s).SS / B;
+                grab_replay(ctx, res, mode, s, ch->run_c0[s], blk0, ch->ended[s], f, counter, k);
                 ch->frame_next[s] = ch->ended[s] ? GrabFrame{} : f; // reset_sdr_flow()
                 ch->counter_next[s] = counter;
             }
@@ -2929,7 +3046,7 @@ int r433b_grab_copy(r433b_ctx *ctx, r433b_results const *res, uint32_t first, ui
         for (uint32_t i = first; i < first + count; ++i) {
             r433b_grab const &g = ctx->grabs[i];
             auto segments = [&](int64_t a, int64_t b) {
-                if (ctx->chained) chain_grab_segments(ctx, ctx->chain_last, g.stream, a, b, dst, segs);
+                if (ctx->chained) chain_grab_segments(ctx, ctx->chain_last, g.stream, a, b, dst, segs, seg_stream);
                 else grab_segments(ctx, a, b, dst, segs, seg_stream);
             };
             int64_t const lo = g.run_end - (int64_t)g.bytes, hi = g.run_end;

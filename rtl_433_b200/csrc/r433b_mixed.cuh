@@ -2,9 +2,10 @@
 // class launches back in order.  The launches append to one package arena in completion order, interleaved; k_slice2
 // needs one contiguous package range per sample rate.  Three passes of the same kernel: count the packages of every
 // internal stream, scan the counts in internal order (streams sorted by class, so every rate slot is one run of them),
-// scatter every header to base[stream] + seq with the caller's stream index.  A stream's packages of one batch have
-// seq 0 .. count - 1, so the order is (internal stream, seq) whatever order the launches stored them in.  The widths stay
-// in the pools (pulse_off is kept).
+// scatter every header to base[stream] + seq - start_seq[stream] with the caller's stream index.  A stream's packages of
+// one batch have seq start_seq .. start_seq + count - 1 (start_seq: 0, or the seq a chain slot carried in), so the order
+// is (internal stream, seq) whatever order the launches stored them in.  The widths stay in the pools (pulse_off is
+// kept).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -22,6 +23,7 @@ struct MixedOrder {
     unsigned n_streams;       // internal streams
     unsigned const *caller;   // caller's index of internal stream s
     unsigned *base;           // n_streams + 1: packages per stream (pass 0), then their first position (pass 1)
+    unsigned const *start_seq; // seq of internal stream s's first package of the batch; nullptr: 0 (unchained)
 };
 
 // pass 0: count (grid-stride, base zeroed by the host); pass 1: exclusive scan in place (one warp); pass 2: scatter
@@ -50,7 +52,7 @@ __global__ void __launch_bounds__(kMixedThreads) k_mixed_order(MixedOrder m, int
             atomicAdd(&m.base[m.src[i].stream], 1u);
         } else {
             r433b_package k = m.src[i];
-            unsigned const at = m.base[k.stream] + k.seq;
+            unsigned const at = m.base[k.stream] + k.seq - (m.start_seq ? m.start_seq[k.stream] : 0u);
             k.stream = m.caller[k.stream];
             m.dst[at] = k;
         }

@@ -33,7 +33,8 @@ EXPORTS = ["r433b_create", "r433b_destroy", "r433b_last_error", "r433b_set_level
            "r433b_dispatch_r_devices_parallel", "r433b_analyze", "r433b_analysis_get", "r433b_analysis_text",
            "r433b_analysis_events", "r433b_submit", "r433b_wait", "r433b_grab_plan", "r433b_grab_copy", "r433b_grab_tail",
            "r433b_chain_create", "r433b_chain_destroy", "r433b_process_chained", "r433b_chain_base",
-           "r433b_chain_grab", "r433b_set_split", "r433b_chain_split", "r433b_process_mixed"]
+           "r433b_chain_grab", "r433b_set_split", "r433b_chain_split", "r433b_process_mixed",
+           "r433b_process_mixed_chained"]
 
 
 def build(force=False, verbose=False):
@@ -178,6 +179,7 @@ def load():
     L.r433b_set_r_devices.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
     L.r433b_process.argtypes = [C.c_void_p, C.POINTER(Batch)]
     L.r433b_process_mixed.argtypes = [C.c_void_p, C.POINTER(Batch), C.POINTER(StreamFormat)]
+    L.r433b_process_mixed_chained.argtypes = [C.c_void_p, C.POINTER(Batch), C.POINTER(StreamFormat), C.c_void_p, C.c_void_p]
     L.r433b_chain_create.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_void_p)]
     L.r433b_chain_destroy.argtypes = [C.c_void_p]
     L.r433b_process_chained.argtypes = [C.c_void_p, C.POINTER(Batch), C.c_void_p, C.c_void_p]
@@ -504,9 +506,11 @@ class Context:
         return a, g, buf.value.decode(), bbs
 
     def process_mixed(self, data, offsets, formats, rates, freqs, lengths=None, fpdm_mode=FPDM_AUTO, data_on_device=False,
-                      block_bytes=0):
+                      block_bytes=0, chain=None, last=None):
         """A batch whose stream i has its own sample format, rate and centre frequency (formats[i], rates[i], freqs[i];
-        include/r433b.h: r433b_process_mixed).  `data`: host numpy array or an int device pointer."""
+        include/r433b.h: r433b_process_mixed).  `data`: host numpy array or an int device pointer.  With a Chain, stream
+        i is the next chunk of slot i's file and `last[i]` says whether the file ends with it
+        (r433b_process_mixed_chained)."""
         offs = np.ascontiguousarray(offsets, dtype=np.uint64)
         n = len(offs) - 1
         if not (len(formats) == len(rates) == len(freqs) == n):
@@ -523,7 +527,11 @@ class Context:
         b = Batch(ptr, offs.ctypes.data_as(C.POINTER(C.c_uint64)), n, 0, 0, 0, fpdm_mode, block_bytes, int(data_on_device), 0,
                   None if lens is None else lens.ctypes.data_as(C.POINTER(C.c_uint64)))
         self._keep = (data, offs, lens)
-        self._check(self.L.r433b_process_mixed(self.h, C.byref(b), fmt))
+        if chain is None:
+            self._check(self.L.r433b_process_mixed(self.h, C.byref(b), fmt))
+            return
+        flags = np.ascontiguousarray(np.ones(n) if last is None else last, dtype=np.uint8)
+        self._check(self.L.r433b_process_mixed_chained(self.h, C.byref(b), fmt, chain.h, flags.ctypes.data))
 
     def submit(self, data, offsets, sample_format, samp_rate=250000, center_frequency=433920000, fpdm_mode=FPDM_AUTO,
                block_bytes=0, data_on_device=False, lengths=None):
