@@ -151,8 +151,8 @@ int r433b_set_fm_low_pass(r433b_ctx *ctx, float fm_low_pass);
 int r433b_set_pipeline(r433b_ctx *ctx, int groups);
 
 /* Segmented replay: k_detect walks one stream with one warp, so a batch of a few long captures leaves most of the GPU
-   idle.  With splitting on, r433b_process() (and r433b_submit()) cuts each long stream at block boundaries into
-   segments of segment_blocks blocks and walks them on separate warps:
+   idle.  With splitting on, r433b_process() (and r433b_submit()) and r433b_process_mixed() cut each long stream at
+   block boundaries into segments of segment_blocks blocks and walk them on separate warps:
    - pass 0 walks, as a file start, the warmup_blocks blocks in front of every segment but a stream's first; its end
      state is the segment's seed (the state the detector would have had the recording begun there);
    - pass 1 walks every segment, the first from the file start and every other from its seed;
@@ -211,14 +211,22 @@ int r433b_process(r433b_ctx *ctx, r433b_batch const *batch);
      ascend and stream i fills its gap; with lengths, stream i is [offsets[i], offsets[i] + lengths[i]), which must end by
      offsets[n_streams], and the offsets need not ascend.
    - want_stages returns R433B_EINVAL.  There is no asynchronous (r433b_submit) form; the chained form is
-     r433b_process_mixed_chained() below.  A mixed batch runs unsplit whatever r433b_set_split says, and host input
-     goes to the device in one copy, without time slices (r433b_set_pipeline).
+     r433b_process_mixed_chained() below.  Host input goes to the device in one copy, without time slices
+     (r433b_set_pipeline).
    - Streams that one detector launch can walk together (the same sample size after load-time conversion, cs8 flip,
      rate and resolved FPDM) form a class.  Each class is one launch of k_front and k_detect; the launches run
      side by side on a small pool of CUDA streams.  r433b_timing: front_ms is the wall time from the first launch to
      the end of the last k_front, detect_ms from the start of the first k_detect to the end of the last; mixed_classes
      counts the classes, detect_launches the launches (a class whose streams lie in two device buffers, the caller's
      and that of the converted cf32 streams, takes one per buffer).
+   - r433b_set_split applies as to r433b_process(): the segments are cut from every stream's bytes after conversion,
+     in whole blocks, and R433B_SPLIT_AUTO counts the blocks of all streams.  Every pass (warm-ups, segments) and every
+     rewalk round launches each class with segments in it once, side by side as above, and a round takes the first
+     rejected segment of every stream of every class.  The results are those of the unsplit mixed batch, bit for bit.
+     r433b_timing of a split mixed batch: split_segments, split_rewalks, split_rounds and split_merge_ms as for
+     r433b_set_split; detect_launches and front_launches count the class launches of every pass and round, those of
+     attempts that overflowed the arenas included; front_ms and detect_ms add up the spans above over the passes;
+     mixed_classes is that of the unsplit batch; mixed_order_ms is 0 (the merge leaves the packages in rate order).
    - Afterwards everything works as after r433b_process(), and every value refers to the stream's own format, rate and
      centre frequency: fetch, digests, r433b_package_to_pulse_data(), r433b_package_file_pos(), the dispatch calls,
      the analyzer and the grabber.  The grabber's run is every stream's used bytes in the caller's order, so a window

@@ -1120,6 +1120,88 @@ int run_sequential(r433b_ctx *ctx, r433b_batch const *b, Shape const &s, DetectP
     return R433B_OK;
 }
 
+// ---- detector launches per class (DESIGN §7d) -----------------------------------------------------------------------
+
+// A class: the streams one detector launch can walk together, and the device buffer they lie in (bufs[buf] of the
+// launch).  A mixed batch's internal order sorts its streams by class, stable in the caller's; a class is the streams
+// [begin, end) of a launch view.  A one-format batch is one class.
+struct MixedClass {
+    uint32_t rate, SS, flip, fpdm, buf;
+    uint32_t begin, end;
+    uint64_t max_samples;
+    bool same(MixedClass const &o) const
+    {
+        return rate == o.rate && SS == o.SS && flip == o.flip && fpdm == o.fpdm && buf == o.buf;
+    }
+};
+
+// The classes of a batch over its streams in internal order, the two device buffers they read (the caller's, the cf32
+// conversion region), and the first internal stream of every sample rate's slot, + n_streams: k_slice2's ranges
+struct ClassSet {
+    std::vector<MixedClass> classes;
+    uint8_t const *bufs[2];
+    std::vector<uint32_t> rate_first;
+};
+
+float elapsed_ms(cudaEvent_t a, cudaEvent_t b)
+{
+    float t = 0;
+    cudaEventElapsedTime(&t, a, b);
+    return t;
+}
+
+// One k_front + k_detect launch per class over the launch view in `dp`, each with its class's buffer, format and FM
+// filter, round-robin on the CUDA stream pool behind everything stream 0 has queued; stream 0 waits for every launch.
+// ev[4]: the start; ev_mx[2c] / ev_mx[2c + 1]: class c's k_front / k_detect done.
+int launch_classes(r433b_ctx *ctx, DetectParams const &dp, std::vector<MixedClass> const &classes,
+        uint8_t const *const bufs[2], uint32_t block_bytes)
+{
+    cudaStream_t const st = 0;
+    while (ctx->ev_mx.size() < 2 * classes.size()) {
+        cudaEvent_t e;
+        CU(cudaEventCreate(&e));
+        ctx->ev_mx.push_back(e);
+    }
+    CU(cudaEventRecord(ctx->ev[4], st));
+    for (size_t c = 0; c < classes.size(); ++c) {
+        MixedClass const &k = classes[c];
+        cudaStream_t const ps = ctx->s_mx[c % r433b_ctx::kMixedStreams];
+        DetectParams q = dp;
+        q.data = bufs[k.buf];
+        q.stream0 = k.begin;
+        q.stream_end = k.end;
+        q.flip = k.flip;
+        q.fpdm = (int)k.fpdm;
+        q.rate = k.rate;
+        q.block_samples = block_bytes / k.SS;
+        set_fm_filter(ctx, (int)k.SS, q);
+        Shape sh{};
+        sh.SS = (int)k.SS;
+        sh.max_samples = k.max_samples;
+        CU(cudaStreamWaitEvent(ps, ctx->ev[4], 0));
+        launch_detect(ctx, q, sh, ps, ctx->ev_mx[2 * c]);
+        CU(cudaGetLastError());
+        CU(cudaEventRecord(ctx->ev_mx[2 * c + 1], ps));
+        CU(cudaStreamWaitEvent(st, ctx->ev_mx[2 * c + 1], 0));
+    }
+    return R433B_OK;
+}
+
+// The spans of the last launch_classes() of `n` classes, once it has completed: k_front from the start to the last
+// class's k_front end, k_detect from the first class's k_detect start to the last one's end
+void class_spans(r433b_ctx const *ctx, size_t n, float &front_ms, float &detect_ms)
+{
+    float front_end = 0, detect_begin = 0, detect_end = 0;
+    for (size_t c = 0; c < n; ++c) {
+        float const f = elapsed_ms(ctx->ev[4], ctx->ev_mx[2 * c]), d = elapsed_ms(ctx->ev[4], ctx->ev_mx[2 * c + 1]);
+        front_end = std::max(front_end, f);
+        detect_begin = c ? std::min(detect_begin, f) : f;
+        detect_end = std::max(detect_end, d);
+    }
+    front_ms = front_end;
+    detect_ms = detect_end - detect_begin;
+}
+
 // ---- segmented replay (r433b_set_split, DESIGN §7c) ---------------------------------------------------------------
 
 // The segments of a batch, stream by stream: segment k is bytes [begin, begin + bytes) of batch stream `stream`
@@ -1130,10 +1212,10 @@ struct SplitPlan {
 };
 
 // Segments of segment_blocks blocks (R433B_SPLIT_AUTO: chosen from the batch) behind warm-ups of warmup_blocks, cut from
-// each stream's used bytes (a chained batch's: each slot's chunk).  false: the batch runs unsplit (splitting off, stage
-// arrays, or no stream of two segments).
+// each stream's used bytes (a chained batch's: each slot's chunk), stream by stream in `order` (a mixed batch's internal
+// order; null: the batch's).  false: the batch runs unsplit (splitting off, stage arrays, or no stream of two segments).
 bool plan_split(r433b_ctx const *ctx, r433b_batch const *b, Shape const &s, uint32_t segment_blocks, uint32_t warmup_blocks,
-        SplitPlan &p)
+        SplitPlan &p, std::vector<uint32_t> const *order = nullptr)
 {
     if (!segment_blocks || b->want_stages || !b->n_streams) return false;
     uint64_t const bb = s.settings.block_bytes;
@@ -1148,7 +1230,8 @@ bool plan_split(r433b_ctx const *ctx, r433b_batch const *b, Shape const &s, uint
     }
     p.warmup = std::min<uint64_t>(warmup_blocks, seg);
     bool any = false;
-    for (uint32_t i = 0; i < b->n_streams; ++i) {
+    for (uint32_t j = 0; j < b->n_streams; ++j) {
+        uint32_t const i = order ? (*order)[j] : j;
         uint64_t const len = ctx->lengths[i], blocks = (len + bb - 1) / bb;
         uint32_t const first = (uint32_t)p.stream.size();
         bool const split = blocks > seg && blocks >= min_blocks;
@@ -1163,40 +1246,55 @@ bool plan_split(r433b_ctx const *ctx, r433b_batch const *b, Shape const &s, uint
     return any;
 }
 
-// The streams of one launch of the split schedule: stream i walks bytes [off, off + len) of the batch's data as a chained
-// chunk whose sample 0 is absolute sample `base` of its file, from the state it holds where `cont`, flushing where `last`
+// The streams of one pass of the split schedule: stream i walks bytes [off, off + len) of its class's buffer as a
+// chained chunk whose sample 0 is absolute sample `base` of its file, from the state it holds where `cont`, flushing
+// where `last`.  `cls`: its class; the streams of a class are consecutive.
 struct SplitLaunch {
     std::vector<uint64_t> off, len, base;
     std::vector<uint8_t> cont, last;
-    void add(uint64_t o, uint64_t l, uint64_t b0, bool c, bool e)
+    std::vector<uint32_t> cls;
+    void add(uint64_t o, uint64_t l, uint64_t b0, bool c, bool e, uint32_t k)
     {
         off.push_back(o);
         len.push_back(l);
         base.push_back(b0);
         cont.push_back(c ? 1 : 0);
         last.push_back(e ? 1 : 0);
+        cls.push_back(k);
     }
 };
 
-// k_front and k_detect over one launch's streams with `state` / `train` as their chain state; the counters are read back
-// into `cnt` (they go on from the launch before)
-int split_launch(r433b_ctx *ctx, DetectParams const &dp, Shape const &s, SplitLaunch const &v, StreamState *state,
-        int *train, DetectCounters &cnt, float &front_ms, float &detect_ms)
+// What the passes of a split batch add up: class launches, the k_front and k_detect spans
+struct SplitTotals {
+    unsigned launches = 0;
+    float front_ms = 0, detect_ms = 0;
+};
+
+// One pass: its view to the device, then k_front and k_detect per class with streams in it (launch_classes) with
+// `state` / `train` as their chain state; the counters are read back into `cnt` (they go on from the pass before)
+int split_launch(r433b_ctx *ctx, DetectParams const &dp, Shape const &s, ClassSet const &cs, SplitLaunch const &v,
+        StreamState *state, int *train, DetectCounters &cnt, SplitTotals &tot)
 {
     cudaStream_t const st = 0;
     size_t const n = v.off.size();
     if (!n) return R433B_OK;
     std::vector<uint64_t> view(4 * n + 2); // offsets (n + 1), lengths, AM offsets (n + 1), bases
     uint64_t *off = view.data(), *len = off + n + 1, *amoff = len + n, *base = amoff + n + 1;
-    Shape sh = s;
-    sh.max_samples = 0;
+    std::vector<MixedClass> runs; // the pass's class launches: the view's runs of one class
     amoff[0] = 0;
     for (size_t i = 0; i < n; ++i) {
+        MixedClass const &k = cs.classes[v.cls[i]];
+        if (i == 0 || v.cls[i] != v.cls[i - 1]) {
+            runs.push_back(k);
+            runs.back().begin = (uint32_t)i;
+            runs.back().max_samples = 0;
+        }
+        runs.back().end = (uint32_t)i + 1;
+        runs.back().max_samples = std::max<uint64_t>(runs.back().max_samples, v.len[i] / k.SS);
         off[i] = v.off[i];
         len[i] = v.len[i];
         base[i] = v.base[i];
-        amoff[i + 1] = amoff[i] + (v.len[i] / s.SS + kTile - 1) / kTile * kTile;
-        sh.max_samples = std::max<uint64_t>(sh.max_samples, v.len[i] / s.SS);
+        amoff[i + 1] = amoff[i] + (v.len[i] / k.SS + kTile - 1) / kTile * kTile;
     }
     off[n] = s.total_bytes;
     std::vector<uint8_t> flags(v.cont);
@@ -1215,17 +1313,14 @@ int split_launch(r433b_ctx *ctx, DetectParams const &dp, Shape const &s, SplitLa
     q.state = state;
     q.train_scratch = train;
     q.fm_out = nullptr;
-    CU(cudaEventRecord(ctx->ev_t[0], st));
-    launch_detect(ctx, q, sh, st, ctx->ev_t[1]);
-    CU(cudaGetLastError());
+    if (int r = launch_classes(ctx, q, runs, cs.bufs, s.settings.block_bytes)) return r;
     CU(cudaMemcpyAsync(&cnt, ctx->d_counters.p, sizeof(cnt), cudaMemcpyDeviceToHost, st));
-    CU(cudaEventRecord(ctx->ev_t[2], st));
-    CU(cudaEventSynchronize(ctx->ev_t[2]));
-    float a = 0, d = 0;
-    cudaEventElapsedTime(&a, ctx->ev_t[0], ctx->ev_t[1]);
-    cudaEventElapsedTime(&d, ctx->ev_t[1], ctx->ev_t[2]);
-    front_ms += a;
-    detect_ms += d;
+    CU(cudaStreamSynchronize(st));
+    float f = 0, d = 0;
+    class_spans(ctx, runs.size(), f, d);
+    tot.front_ms += f;
+    tot.detect_ms += d;
+    tot.launches += (unsigned)runs.size();
     return R433B_OK;
 }
 
@@ -1249,14 +1344,16 @@ int split_compare(r433b_ctx *ctx, std::vector<uint32_t> const &segs, std::vector
     return R433B_OK;
 }
 
-// The split schedule on stream 0: copy-in, pass 0 (warm-ups -> seeds), pass 1 (every segment), rounds of rewalks until
-// every segment has started from its predecessor's exact end state, the merge, then the slicers over the merged packages.
-// An arena overflow in any launch grows the caps from what the device counted and runs the schedule again from pass 0.
-// With a chain, stream i's segments lie at the chain's base for slot i, the first starts from the state the chain
-// carried (loaded in front of pass 1, so a rerun loads it again), the last ends as the chunk does (last[i]), and the
-// chain takes the last's end state once everything has succeeded.
-int run_split(r433b_ctx *ctx, r433b_batch const *b, Shape const &s, SplitPlan const &p, DetectParams const &dp0,
-        r433b_chain *ch, uint8_t const *last_chunk, DetectCounters &cnt)
+// The split schedule on stream 0, behind the copy-in: pass 0 (warm-ups -> seeds), pass 1 (every segment), rounds of
+// rewalks until every segment has started from its predecessor's exact end state, the merge, then the slicers over the
+// merged packages, one range per sample rate.  Every pass and round launches each class with segments in it once
+// (`cs`; the plan is in the classes' internal order), so a round takes the first rejected segment of every stream of
+// every class.  An arena overflow in any pass grows the caps from what the device counted and runs the schedule again
+// from pass 0.  With a chain, stream i's segments lie at the chain's base for slot i, the first starts from the state
+// the chain carried (loaded in front of pass 1, so a rerun loads it again), the last ends as the chunk does (last[i]),
+// and the chain takes the last's end state once everything has succeeded.
+int run_split(r433b_ctx *ctx, r433b_batch const *b, Shape const &s, SplitPlan const &p, ClassSet const &cs,
+        DetectParams const &dp0, r433b_chain *ch, uint8_t const *last_chunk, DetectCounters &cnt)
 {
     cudaStream_t const st = 0;
     size_t const n = p.stream.size(), ns = b->n_streams, tr = (size_t)kTrainInts * sizeof(int);
@@ -1275,36 +1372,36 @@ int run_split(r433b_ctx *ctx, r433b_batch const *b, Shape const &s, SplitPlan co
     DetectParams dp = dp0;
     dp.log_scratch = (unsigned *)ctx->d_log.p;
 
-    CU(cudaEventRecord(ctx->ev[0], st));
-    if (int r = copy_in(ctx, b, s, st)) return r;
-    CU(cudaEventRecord(ctx->ev[1], st));
-
     // pass 0 walks the warm-up in front of every segment but a stream's first (those slots walk nothing), pass 1 the
     // segments; slot k is segment k in both
     SplitLaunch warm, walk;
     std::vector<uint32_t> later, slots(2 * ns); // every segment but a stream's first; each stream's first and last
-    for (size_t k = 0; k < n; ++k) {
+    std::vector<uint32_t> stream_seg;           // the first segment of internal stream j, + n
+    for (size_t k = 0, c = 0; k < n; ++k) {
         uint32_t const i = p.stream[k];
         bool const first = p.first[k] == k, last = k + 1 == n || p.first[k + 1] != p.first[k];
+        if (first) stream_seg.push_back((uint32_t)k);
+        while (cs.classes[c].end < stream_seg.size()) ++c;
+        uint64_t const SS = cs.classes[c].SS;
         uint64_t const o = ctx->offsets[i], w0 = first || p.begin[k] < p.warmup * bb ? 0 : p.begin[k] - p.warmup * bb;
         uint64_t const base = ch ? ctx->chain_base[i] : 0;
-        warm.add(o + w0, first ? 0 : p.begin[k] - w0, base + w0 / s.SS, false, false);
-        walk.add(o + p.begin[k], p.bytes[k], base + p.begin[k] / s.SS, first ? ch && ch->open[i] : true,
-                 last && (!ch || last_chunk[i]));
+        warm.add(o + w0, first ? 0 : p.begin[k] - w0, base + w0 / SS, false, false, (uint32_t)c);
+        walk.add(o + p.begin[k], p.bytes[k], base + p.begin[k] / SS, first ? ch && ch->open[i] : true,
+                 last && (!ch || last_chunk[i]), (uint32_t)c);
         if (!first) later.push_back((uint32_t)k);
         if (first) slots[i] = (uint32_t)k;
         if (last) slots[ns + i] = (uint32_t)k;
     }
+    stream_seg.push_back((uint32_t)n);
     if (ch) CU(cudaMemcpyAsync(slot_first, slots.data(), 2 * ns * sizeof(unsigned), cudaMemcpyHostToDevice, st));
-    float front_ms = 0, detect_ms = 0;
-    unsigned launches = 0, rewalks = 0, rounds = 0;
+    SplitTotals tot;
+    unsigned rewalks = 0, rounds = 0;
     DetectCounters warm_cnt{};
     std::vector<uint32_t> final_walk, launch_lo, map_off, seg_of;
     for (int attempt = 0;; ++attempt) {
         if (int r = bind_detector_arenas(ctx, dp)) return r;
         CU(cudaMemsetAsync(ctx->d_counters.p, 0, 64, st));
-        if (int r = split_launch(ctx, dp, s, warm, state, train, warm_cnt, front_ms, detect_ms)) return r;
-        launches++;
+        if (int r = split_launch(ctx, dp, s, cs, warm, state, train, warm_cnt, tot)) return r;
         // the warm-ups' packages are not kept: the arenas start again behind them
         CU(cudaMemsetAsync(ctx->d_counters.p, 0, 64, st));
         CU(cudaMemcpyAsync(ctx->d_sp_seed.p, state, n * sizeof(StreamState), cudaMemcpyDeviceToDevice, st));
@@ -1321,8 +1418,7 @@ int run_split(r433b_ctx *ctx, r433b_batch const *b, Shape const &s, SplitPlan co
                       (int *)ctx->d_sp_seed_train.p, (unsigned)n);
             CU(cudaGetLastError());
         }
-        if (int r = split_launch(ctx, dp, s, walk, state, train, cnt, front_ms, detect_ms)) return r;
-        launches++;
+        if (int r = split_launch(ctx, dp, s, cs, walk, state, train, cnt, tot)) return r;
         final_walk.assign(n, 0);
         launch_lo = {0, cnt.pkgs};
         map_off = {0};
@@ -1351,10 +1447,9 @@ int run_split(r433b_ctx *ctx, r433b_batch const *b, Shape const &s, SplitPlan co
             R4_LAUNCH(k_split_gather, grid, kSplitWarps * 32, 0, st, (StreamState const *)state, (int const *)train,
                       (unsigned const *)list, m, rw_state, rw_train, start_seq);
             CU(cudaGetLastError());
-            SplitLaunch again;
-            for (uint32_t k : rw) again.add(walk.off[k], walk.len[k], walk.base[k], true, walk.last[k] != 0);
-            if (int r = split_launch(ctx, dp, s, again, rw_state, rw_train, cnt, front_ms, detect_ms)) return r;
-            launches++;
+            SplitLaunch again; // rw ascends, so its classes stay consecutive
+            for (uint32_t k : rw) again.add(walk.off[k], walk.len[k], walk.base[k], true, walk.last[k] != 0, walk.cls[k]);
+            if (int r = split_launch(ctx, dp, s, cs, again, rw_state, rw_train, cnt, tot)) return r;
             R4_LAUNCH(k_split_scatter, grid, kSplitWarps * 32, 0, st, (StreamState const *)rw_state, (int const *)rw_train,
                       (unsigned const *)list, m, state, train);
             CU(cudaGetLastError());
@@ -1378,7 +1473,9 @@ int run_split(r433b_ctx *ctx, r433b_batch const *b, Shape const &s, SplitPlan co
         if (attempt == 2) return fail(ctx, R433B_EOVERFLOW, "package arena overflow");
     }
 
-    // the merge: the packages of every segment's last walk, renumbered, into a second set of arenas that then swaps in
+    // the merge: the packages of every segment's last walk, renumbered, into a second set of arenas that then swaps in.
+    // Segments are in internal order and carry the batch's stream index, so the merged packages are in (internal
+    // stream, seq) order: every sample rate's streams are one range.
     size_t const n_launch = launch_lo.size() - 1, n_src = launch_lo.back();
     std::vector<uint32_t> tab;
     tab.reserve(3 * n + 2 * n_launch + 1 + seg_of.size() + 1);
@@ -1419,19 +1516,23 @@ int run_split(r433b_ctx *ctx, r433b_batch const *b, Shape const &s, SplitPlan co
     if (n_src) R4_LAUNCH(k_split_merge, (unsigned)((n_src + kSplitWarps - 1) / kSplitWarps), kSplitWarps * 32, 0, st, mg);
     CU(cudaGetLastError());
     CU(cudaEventRecord(ctx->ev_t[4], st));
-    unsigned kept[2] = {0, 0}; // packages, pool entries
-    CU(cudaMemcpyAsync(&kept[0], pkg_base + n, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(&kept[1], mg.pool_cursor, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+    std::vector<unsigned> merged(n + 1); // pkg_base: where each segment's packages start, + the total
+    unsigned pool_kept = 0;
+    CU(cudaMemcpyAsync(merged.data(), pkg_base, (n + 1) * sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(&pool_kept, mg.pool_cursor, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     std::swap(ctx->d_pkgs, ctx->d_sp_pkgs);
     std::swap(ctx->d_ppool, ctx->d_sp_ppool);
     std::swap(ctx->d_gpool, ctx->d_sp_gpool);
-    if (int r = check_pair_index(ctx, kept[0])) return r;
-    ctx->n_pkgs = kept[0];
-    ctx->pool_used = kept[1];
-    GroupRange all{};
-    all.pkg_end = ctx->n_pkgs;
-    if (int r = slice_ranges(ctx, std::vector<GroupRange>{all}, ctx->n_pkgs, ctx->pool_used, st)) return r;
+    if (int r = check_pair_index(ctx, merged[n])) return r;
+    ctx->n_pkgs = merged[n];
+    ctx->pool_used = pool_kept;
+    std::vector<GroupRange> ranges(cs.rate_first.size() - 1);
+    for (size_t g = 0; g < ranges.size(); ++g) {
+        ranges[g].pkg_begin = merged[stream_seg[cs.rate_first[g]]];
+        ranges[g].pkg_end = merged[stream_seg[cs.rate_first[g + 1]]];
+    }
+    if (int r = slice_ranges(ctx, ranges, ctx->n_pkgs, ctx->pool_used, st)) return r;
     if (ch) {
         R4_LAUNCH(k_split_chain_out, (unsigned)((ns + kSplitWarps - 1) / kSplitWarps), kSplitWarps * 32, 0, st,
                   (StreamState const *)state, (int const *)train, (unsigned const *)slot_first, (unsigned const *)slot_last,
@@ -1450,9 +1551,9 @@ int run_split(r433b_ctx *ctx, r433b_batch const *b, Shape const &s, SplitPlan co
     cudaEventElapsedTime(&ctx->timing.h2d_ms, ctx->ev[0], ctx->ev[1]);
     cudaEventElapsedTime(&ctx->timing.split_merge_ms, ctx->ev_t[3], ctx->ev_t[4]);
     cudaEventElapsedTime(&ctx->timing.total_ms, ctx->ev[0], ctx->ev[3]);
-    ctx->timing.front_ms = front_ms;
-    ctx->timing.detect_ms = detect_ms;
-    ctx->timing.detect_launches = launches;
+    ctx->timing.front_ms = tot.front_ms;
+    ctx->timing.detect_ms = tot.detect_ms;
+    ctx->timing.detect_launches = tot.launches;
     ctx->timing.split_segments = (uint32_t)n;
     ctx->timing.split_rewalks = rewalks;
     ctx->timing.split_rounds = rounds;
@@ -1484,7 +1585,12 @@ int process_iq(r433b_ctx *ctx, r433b_batch const *b, r433b_chain *ch, uint8_t co
     // a chain splits only when it opted in (r433b_chain_split): the context's setting is for unchained batches
     uint32_t const split_blocks = ch ? ch->split_blocks : ctx->split_blocks, split_warmup = ch ? ch->split_warmup : ctx->split_warmup;
     if (plan_split(ctx, b, s, split_blocks, split_warmup, plan)) {
-        r = run_split(ctx, b, s, plan, dp, ch, last, cnt);
+        ClassSet const cs{{MixedClass{b->samp_rate, (uint32_t)s.SS, (uint32_t)dp.flip, s.fmt.fpdm, 0, 0, b->n_streams, s.max_samples}},
+                          {dp.data, dp.data}, {0, b->n_streams}};
+        CU(cudaEventRecord(ctx->ev[0], 0));
+        r = copy_in(ctx, b, s, 0);
+        CU(cudaEventRecord(ctx->ev[1], 0));
+        if (!r) r = run_split(ctx, b, s, plan, cs, dp, ch, last, cnt);
     } else {
         uint64_t slice_samples;
         int const G = time_slices(ctx, b, s, slice_samples);
@@ -1507,24 +1613,26 @@ int process_iq(r433b_ctx *ctx, r433b_batch const *b, r433b_chain *ch, uint8_t co
 
 // ---- mixed batches (r433b_process_mixed, DESIGN §7d) -----------------------------------------------------------------
 
-// A class: the streams one detector launch can walk together, and the device buffer they lie in.  The internal order
-// sorts the streams by class, stable in the caller's; a class is the internal streams [begin, end).
-struct MixedClass {
-    uint32_t rate, SS, flip, fpdm, buf;
-    uint32_t begin, end;
-    uint64_t max_samples;
-    bool same(MixedClass const &o) const
-    {
-        return rate == o.rate && SS == o.SS && flip == o.flip && fpdm == o.fpdm && buf == o.buf;
-    }
+// What the setup of a mixed batch leaves to its schedule (the unsplit class launches, or the split schedule)
+struct MixedBatch {
+    ChainSettings settings;
+    std::vector<SlotFormat> slots;   // per caller stream
+    std::vector<uint32_t> order;     // the caller's index of internal stream j
+    ClassSet cs;
+    std::vector<uint32_t> rates;     // distinct rates ascending; rate slot g starts at internal stream cs.rate_first[g]
+    std::vector<uint64_t> conv;      // per caller stream: where its cs16 bytes lie in the conversion region, or UINT64_MAX
+    uint64_t conv_base = 0, n_samples = 0;
+    uint32_t n_classes = 0;          // distinct (rate, SS, flip, fpdm): launches over both buffers count once
+    unsigned *start_seq = nullptr, *internal_of = nullptr;
+    unsigned char *slot_cont = nullptr;
+    DetectParams dp{};
 };
 
-// rtl_433 -r f1 -r f2 ... on a batch of files of their own formats: one k_front + k_detect launch per class on the
-// CUDA stream pool, k_mixed_order, then the slicers over one package range per rate.  With a chain, stream i is the
-// next chunk of slot i's file: the slots' state is gathered into internal order in front of every attempt and
-// scattered back once the batch has succeeded (DESIGN §7d).
-int process_mixed(r433b_ctx *ctx, r433b_batch const *b, r433b_stream_format const *fmt, r433b_chain *ch,
-        uint8_t const *last)
+// A mixed batch's arguments, the context's record of the batch, its internal order and classes, the device tables in
+// that order, the slicer tables per rate and the detector's parameters.  With a chain, stream i is the next chunk of
+// slot i's file: chain_begin() permutes its flags and bases.
+int mixed_setup(r433b_ctx *ctx, r433b_batch const *b, r433b_stream_format const *fmt, r433b_chain *ch,
+        uint8_t const *last, MixedBatch &m)
 {
     if (!ctx || !b || !b->offsets || (b->n_streams && (!b->data || !fmt))) return fail(ctx, R433B_EINVAL, "null argument");
     if (b->sample_format || b->samp_rate || b->center_frequency)
@@ -1540,7 +1648,8 @@ int process_mixed(r433b_ctx *ctx, r433b_batch const *b, r433b_stream_format cons
         if (d.modulation >= 16) enable_fm = 1;
     // per stream: checks, its class key, its bytes after conversion (cf32 -> cs16, in the conversion region)
     std::vector<MixedClass> key(n);
-    std::vector<uint64_t> len(n), in_lens(n), conv(n, UINT64_MAX);
+    std::vector<uint64_t> len(n), in_lens(n);
+    m.conv.assign(n, UINT64_MAX);
     uint64_t conv_bytes = 0;
     for (uint32_t i = 0; i < n; ++i) {
         uint32_t const f = fmt[i].sample_format;
@@ -1558,18 +1667,18 @@ int process_mixed(r433b_ctx *ctx, r433b_batch const *b, r433b_stream_format cons
         in_lens[i] = in_len;
         len[i] = in_div == 2 ? in_len / 8 * 4 : in_len; // whole IQ pairs of floats -> cs16 bytes
         if (in_div == 2) {
-            conv[i] = conv_bytes;
+            m.conv[i] = conv_bytes;
             conv_bytes += (len[i] + 15) / 16 * 16;
         }
         uint32_t const fpdm = b->fpdm_mode == R433B_FPDM_AUTO ? (fmt[i].center_frequency > 800000000u ? 1u : 0u) : b->fpdm_mode;
         key[i] = MixedClass{fmt[i].samp_rate, SS, dp_flip_of(f), fpdm, in_div == 2 && b->data_on_device ? 1u : 0u, 0, 0, 0};
     }
-    ChainSettings const settings{block_bytes, ctx->use_mag, enable_fm, ctx->level_limit, ctx->min_level, ctx->min_snr,
-                                 ctx->fm_low_pass};
-    std::vector<SlotFormat> slots(n);
-    for (uint32_t i = 0; i < n; ++i) slots[i] = SlotFormat{fmt[i].sample_format, fmt[i].samp_rate, fmt[i].center_frequency, key[i].fpdm};
+    m.settings = ChainSettings{block_bytes, ctx->use_mag, enable_fm, ctx->level_limit, ctx->min_level, ctx->min_snr,
+                               ctx->fm_low_pass};
+    m.slots.resize(n);
+    for (uint32_t i = 0; i < n; ++i) m.slots[i] = SlotFormat{fmt[i].sample_format, fmt[i].samp_rate, fmt[i].center_frequency, key[i].fpdm};
     if (ch)
-        if (int r = check_chain(ctx, b, ch, last, settings, true, slots, in_lens)) return r;
+        if (int r = check_chain(ctx, b, ch, last, m.settings, true, m.slots, in_lens)) return r;
     CU(cudaSetDevice(ctx->device));
 
     // the batch becomes the context's last one
@@ -1586,38 +1695,40 @@ int process_mixed(r433b_ctx *ctx, r433b_batch const *b, r433b_stream_format cons
     ctx->d2h_done = false;
     // device buffers: host input is copied whole to d_data; the converted cf32 streams follow it there (host input) or
     // fill it (device input)
-    uint64_t const conv_base = b->data_on_device ? 0 : (total + 255) / 256 * 256;
+    m.conv_base = b->data_on_device ? 0 : (total + 255) / 256 * 256;
     if (!b->data_on_device || conv_bytes)
-        if (int r = dev_reserve(ctx, ctx->d_data, conv_base + conv_bytes + 64)) return r;
+        if (int r = dev_reserve(ctx, ctx->d_data, m.conv_base + conv_bytes + 64)) return r;
     uint8_t const *const caller = b->data_on_device ? (uint8_t const *)b->data : (uint8_t const *)ctx->d_data.p;
     uint8_t const *const region = (uint8_t const *)ctx->d_data.p;
+    m.cs.bufs[0] = caller;
+    m.cs.bufs[1] = region;
     ctx->offsets.assign(n + 1, total);
     ctx->lengths = len;
     ctx->mixed.resize(n);
-    uint64_t used = 0, n_samples = 0;
+    uint64_t used = 0;
     for (uint32_t i = 0; i < n; ++i) {
-        bool const cv = conv[i] != UINT64_MAX;
-        ctx->offsets[i] = cv ? conv_base + conv[i] : b->offsets[i];
+        bool const cv = m.conv[i] != UINT64_MAX;
+        ctx->offsets[i] = cv ? m.conv_base + m.conv[i] : b->offsets[i];
         ctx->mixed[i] = r433b_ctx::MixedStream{key[i].SS, fmt[i].samp_rate, fmt[i].center_frequency, key[i].flip,
                                                cv ? region : caller};
         used += len[i];
-        n_samples += len[i] / key[i].SS;
+        m.n_samples += len[i] / key[i].SS;
     }
     ctx->batch.offsets = ctx->offsets.data();
     ctx->batch.lengths = ctx->lengths.data();
 
     // the internal order and the classes; the device reads the offsets, lengths and AM offsets in that order
-    std::vector<uint32_t> order(n);
+    std::vector<uint32_t> &order = m.order;
+    order.resize(n);
     for (uint32_t i = 0; i < n; ++i) order[i] = i;
     auto less = [&](MixedClass const &x, MixedClass const &y) {
         return std::tie(x.rate, x.SS, x.flip, x.fpdm, x.buf) < std::tie(y.rate, y.SS, y.flip, y.fpdm, y.buf);
     };
     std::stable_sort(order.begin(), order.end(), [&](uint32_t x, uint32_t y) { return less(key[x], key[y]); });
-    std::vector<MixedClass> classes;
-    std::vector<uint32_t> rates, slot_first; // distinct rates ascending, and the first internal stream of each
+    std::vector<MixedClass> &classes = m.cs.classes;
+    std::vector<uint32_t> &slot_first = m.cs.rate_first;
     std::vector<uint64_t> view(3 * n + 2);   // offsets (n + 1), lengths, AM offsets (n + 1)
     uint64_t *off = view.data(), *lens = off + n + 1, *amoff = lens + n;
-    std::vector<uint32_t> caller_of(order);
     amoff[0] = 0;
     for (uint32_t j = 0; j < n; ++j) {
         uint32_t const i = order[j];
@@ -1625,8 +1736,8 @@ int process_mixed(r433b_ctx *ctx, r433b_batch const *b, r433b_stream_format cons
             classes.push_back(key[i]);
             classes.back().begin = j;
         }
-        if (rates.empty() || rates.back() != key[i].rate) {
-            rates.push_back(key[i].rate);
+        if (m.rates.empty() || m.rates.back() != key[i].rate) {
+            m.rates.push_back(key[i].rate);
             slot_first.push_back(j);
         }
         classes.back().end = j + 1;
@@ -1637,10 +1748,9 @@ int process_mixed(r433b_ctx *ctx, r433b_batch const *b, r433b_stream_format cons
     }
     off[n] = 0;
     slot_first.push_back(n);
-    uint32_t n_classes = 0;
     for (size_t c = 0; c < classes.size(); ++c)
-        n_classes += c == 0 || !(classes[c].rate == classes[c - 1].rate && classes[c].SS == classes[c - 1].SS
-                                 && classes[c].flip == classes[c - 1].flip && classes[c].fpdm == classes[c - 1].fpdm);
+        m.n_classes += c == 0 || !(classes[c].rate == classes[c - 1].rate && classes[c].SS == classes[c - 1].SS
+                                   && classes[c].flip == classes[c - 1].flip && classes[c].fpdm == classes[c - 1].fpdm);
     uint64_t const am_samples = amoff[n];
     size_t const nn = std::max<size_t>(1, n);
     if (int r = dev_reserve(ctx, ctx->d_offsets, (n + 1) * sizeof(uint64_t))) return r;
@@ -1658,21 +1768,22 @@ int process_mixed(r433b_ctx *ctx, r433b_batch const *b, r433b_stream_format cons
     CU(cudaMemcpy(ctx->d_offsets.p, off, (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice));
     if (n) CU(cudaMemcpy(ctx->d_lengths.p, lens, n * sizeof(uint64_t), cudaMemcpyHostToDevice));
     CU(cudaMemcpy(ctx->d_amoff.p, amoff, (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice));
-    if (n) CU(cudaMemcpy(ctx->d_mx_tab.p, caller_of.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice));
-    unsigned *const start_seq = (unsigned *)ctx->d_mx_tab.p + 2 * n + 1, *const internal_of = start_seq + n;
-    unsigned char *const slot_cont = (unsigned char *)(internal_of + n);
+    if (n) CU(cudaMemcpy(ctx->d_mx_tab.p, order.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    m.start_seq = (unsigned *)ctx->d_mx_tab.p + 2 * n + 1;
+    m.internal_of = m.start_seq + n;
+    m.slot_cont = (unsigned char *)(m.internal_of + n);
     if (ch && n) {
         std::vector<uint32_t> in_of(n);
         for (uint32_t j = 0; j < n; ++j) in_of[order[j]] = j;
-        CU(cudaMemcpy(internal_of, in_of.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice));
-        CU(cudaMemcpy(slot_cont, ch->open.data(), n, cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(m.internal_of, in_of.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(m.slot_cont, ch->open.data(), n, cudaMemcpyHostToDevice));
     }
-    if (int r = upload_slicer_tables(ctx, rates, 0)) return r;
+    if (int r = upload_slicer_tables(ctx, m.rates, 0)) return r;
     ctx->pkg_cap = std::max<size_t>(ctx->pkg_cap, ctx->min_caps[0] ? ctx->min_caps[0] : (size_t)n * 16 + 1024);
     ctx->pool_cap = std::max<size_t>(ctx->pool_cap, ctx->min_caps[1] ? ctx->min_caps[1] : ctx->pkg_cap * 128);
     ctx->arena_cap = std::max<size_t>(ctx->arena_cap, ctx->min_caps[2] ? ctx->min_caps[2] : used / 2 + (1u << 20));
 
-    DetectParams dp{};
+    DetectParams &dp = m.dp;
     dp.offsets = (unsigned long long const *)ctx->d_offsets.p;
     dp.lengths = (unsigned long long const *)ctx->d_lengths.p;
     dp.am_offsets = (unsigned long long const *)ctx->d_amoff.p;
@@ -1690,61 +1801,49 @@ int process_mixed(r433b_ctx *ctx, r433b_batch const *b, r433b_stream_format cons
     dp.am = (int16_t *)ctx->d_am.p;
     dp.chunks = (ChunkInfo const *)ctx->d_chunks.p;
     dp.tile_info = (TileInfo const *)ctx->d_tiles.p;
-    if (int r = chain_begin(ctx, ch, last, dp, &order)) return r;
-    size_t const n_launch = classes.size();
-    while (ctx->ev_mx.size() < 2 * n_launch) {
-        cudaEvent_t e;
-        CU(cudaEventCreate(&e));
-        ctx->ev_mx.push_back(e);
-    }
+    return chain_begin(ctx, ch, last, dp, &order);
+}
 
+// The batch to the device on stream 0 between ev[0] and ev[1]: host input in one copy, every cf32 stream converted into
+// the region.  A rerun after an arena overflow starts behind it.
+int mixed_copy_in(r433b_ctx *ctx, r433b_batch const *b, MixedBatch const &m)
+{
     cudaStream_t const st = 0;
     CU(cudaEventRecord(ctx->ev[0], st));
     Shape whole{};
-    whole.total_bytes = total;
+    whole.total_bytes = b->n_streams ? b->offsets[b->n_streams] : 0;
     if (int r = copy_in(ctx, b, whole, st)) return r; // host input: one copy; device input: nothing
-    for (uint32_t i = 0; i < n; ++i) {
-        size_t const n4 = (size_t)(len[i] / 4 + 1) / 2; // two cs16 samples per group of four floats
-        if (conv[i] == UINT64_MAX || !n4) continue;
+    for (uint32_t i = 0; i < b->n_streams; ++i) {
+        size_t const n4 = (size_t)(ctx->lengths[i] / 4 + 1) / 2; // two cs16 samples per group of four floats
+        if (m.conv[i] == UINT64_MAX || !n4) continue;
         unsigned const grid = (unsigned)std::min<size_t>((size_t)ctx->n_sms * 8, (n4 + 255) / 256);
-        R4_LAUNCH(k_cf32_to_cs16, grid, 256, 0, st, (float4 const *)(caller + b->offsets[i]),
-                  (uint2 *)((uint8_t *)ctx->d_data.p + conv_base + conv[i]), n4);
+        R4_LAUNCH(k_cf32_to_cs16, grid, 256, 0, st, (float4 const *)(m.cs.bufs[0] + b->offsets[i]),
+                  (uint2 *)((uint8_t *)ctx->d_data.p + m.conv_base + m.conv[i]), n4);
         CU(cudaGetLastError());
     }
     CU(cudaEventRecord(ctx->ev[1], st));
-    DetectCounters cnt{};
+    return R433B_OK;
+}
+
+// The unsplit schedule of a mixed batch: one k_front + k_detect launch per class (again with the arenas grown to what
+// the device counted while they overflow), k_mixed_order, then the slicers over one package range per rate.  A chain's
+// slots are gathered into internal order in front of every attempt and scattered back once the batch has succeeded.
+int run_mixed(r433b_ctx *ctx, r433b_batch const *b, MixedBatch &m, r433b_chain *ch, DetectCounters &cnt)
+{
+    cudaStream_t const st = 0;
+    uint32_t const n = b->n_streams;
+    DetectParams &dp = m.dp;
     for (int attempt = 0;; ++attempt) {
         if (int r = bind_detector_arenas(ctx, dp)) return r;
         CU(cudaMemsetAsync(ctx->d_counters.p, 0, 64, st));
         if (ch) { // from the chain, which only the scatter below writes: also where an overflow reruns from
-            CU(cudaMemsetAsync(start_seq, 0, n * sizeof(unsigned), st));
+            CU(cudaMemsetAsync(m.start_seq, 0, n * sizeof(unsigned), st));
             R4_LAUNCH(k_split_chain_in, (n + kSplitWarps - 1) / kSplitWarps, kSplitWarps * 32, 0, st,
-                      (StreamState const *)ch->d_state.p, (int const *)ch->d_train.p, (unsigned char const *)slot_cont,
-                      (unsigned const *)internal_of, n, (StreamState *)dp.state, dp.train_scratch, start_seq);
+                      (StreamState const *)ch->d_state.p, (int const *)ch->d_train.p, (unsigned char const *)m.slot_cont,
+                      (unsigned const *)m.internal_of, n, (StreamState *)dp.state, dp.train_scratch, m.start_seq);
             CU(cudaGetLastError());
         }
-        CU(cudaEventRecord(ctx->ev[4], st)); // the classes start here
-        for (size_t c = 0; c < n_launch; ++c) {
-            MixedClass const &k = classes[c];
-            cudaStream_t const ps = ctx->s_mx[c % r433b_ctx::kMixedStreams];
-            DetectParams q = dp;
-            q.data = k.buf ? region : caller;
-            q.stream0 = k.begin;
-            q.stream_end = k.end;
-            q.flip = k.flip;
-            q.fpdm = (int)k.fpdm;
-            q.rate = k.rate;
-            q.block_samples = block_bytes / k.SS;
-            set_fm_filter(ctx, (int)k.SS, q);
-            Shape sh{};
-            sh.SS = (int)k.SS;
-            sh.max_samples = k.max_samples;
-            CU(cudaStreamWaitEvent(ps, ctx->ev[4], 0));
-            launch_detect(ctx, q, sh, ps, ctx->ev_mx[2 * c]);
-            CU(cudaGetLastError());
-            CU(cudaEventRecord(ctx->ev_mx[2 * c + 1], ps));
-            CU(cudaStreamWaitEvent(st, ctx->ev_mx[2 * c + 1], 0));
-        }
+        if (int r = launch_classes(ctx, dp, m.cs.classes, m.cs.bufs, m.settings.block_bytes)) return r;
         CU(cudaMemcpyAsync(&cnt, ctx->d_counters.p, sizeof(cnt), cudaMemcpyDeviceToHost, st));
         CU(cudaStreamSynchronize(st));
         if (!cnt.overflow) break;
@@ -1769,7 +1868,7 @@ int process_mixed(r433b_ctx *ctx, r433b_batch const *b, r433b_stream_format cons
         mo.n_streams = n;
         mo.caller = (unsigned const *)ctx->d_mx_tab.p;
         mo.base = (unsigned *)ctx->d_mx_tab.p + n;
-        mo.start_seq = ch ? start_seq : nullptr;
+        mo.start_seq = ch ? m.start_seq : nullptr;
         unsigned const grid = (unsigned)std::min<uint64_t>((uint64_t)ctx->n_sms * 4, (ctx->n_pkgs + kMixedThreads - 1) / kMixedThreads);
         CU(cudaMemsetAsync(mo.base, 0, (n + 1) * sizeof(unsigned), st));
         R4_LAUNCH(k_mixed_order, grid, kMixedThreads, 0, st, mo, 0);
@@ -1781,10 +1880,10 @@ int process_mixed(r433b_ctx *ctx, r433b_batch const *b, r433b_stream_format cons
     CU(cudaEventRecord(ctx->ev_t[1], st));
     CU(cudaEventSynchronize(ctx->ev_t[1]));
     std::swap(ctx->d_pkgs, ctx->d_mx_pkgs);
-    std::vector<GroupRange> ranges(rates.size());
-    for (size_t g = 0; g < rates.size(); ++g) {
-        ranges[g].pkg_begin = base[slot_first[g]];
-        ranges[g].pkg_end = base[slot_first[g + 1]];
+    std::vector<GroupRange> ranges(m.rates.size());
+    for (size_t g = 0; g < m.rates.size(); ++g) {
+        ranges[g].pkg_begin = base[m.cs.rate_first[g]];
+        ranges[g].pkg_end = base[m.cs.rate_first[g + 1]];
     }
     if (int r = slice_ranges(ctx, ranges, ctx->n_pkgs, ctx->pool_used, st)) return r;
     if (ch && n) { // the batch has succeeded: the walks' end states back to their slots
@@ -1794,30 +1893,44 @@ int process_mixed(r433b_ctx *ctx, r433b_batch const *b, r433b_stream_format cons
         CU(cudaGetLastError());
     }
 
-    auto ms = [](cudaEvent_t a, cudaEvent_t e) { float t = 0; cudaEventElapsedTime(&t, a, e); return t; };
-    float front_end = 0, detect_begin = 0, detect_end = 0;
-    for (size_t c = 0; c < n_launch; ++c) {
-        float const f = ms(ctx->ev[4], ctx->ev_mx[2 * c]), d = ms(ctx->ev[4], ctx->ev_mx[2 * c + 1]);
-        front_end = std::max(front_end, f);
-        detect_begin = c ? std::min(detect_begin, f) : f;
-        detect_end = std::max(detect_end, d);
+    class_spans(ctx, m.cs.classes.size(), ctx->timing.front_ms, ctx->timing.detect_ms);
+    ctx->timing.h2d_ms = elapsed_ms(ctx->ev[0], ctx->ev[1]);
+    ctx->timing.total_ms = elapsed_ms(ctx->ev[0], ctx->ev[3]);
+    ctx->timing.mixed_order_ms = elapsed_ms(ctx->ev_t[0], ctx->ev_t[1]);
+    ctx->timing.detect_launches = (uint32_t)m.cs.classes.size();
+    return R433B_OK;
+}
+
+// rtl_433 -r f1 -r f2 ... on a batch of files of their own formats (DESIGN §7d).  Unchained, with splitting on
+// (r433b_set_split) and a stream of two segments, the split schedule walks the segments of every class in the same
+// passes; otherwise every class is one launch.  With a chain, stream i is the next chunk of slot i's file; a chain
+// runs unsplit.
+int process_mixed(r433b_ctx *ctx, r433b_batch const *b, r433b_stream_format const *fmt, r433b_chain *ch,
+        uint8_t const *last)
+{
+    MixedBatch m;
+    if (int r = mixed_setup(ctx, b, fmt, ch, last, m)) return r;
+    if (int r = mixed_copy_in(ctx, b, m)) return r;
+    DetectCounters cnt{};
+    Shape s{};
+    s.settings = m.settings;
+    SplitPlan plan;
+    if (!ch && plan_split(ctx, b, s, ctx->split_blocks, ctx->split_warmup, plan, &m.order)) {
+        if (int r = run_split(ctx, b, s, plan, m.cs, m.dp, nullptr, nullptr, cnt)) return r;
+    } else if (int r = run_mixed(ctx, b, m, ch, cnt)) {
+        return r;
     }
-    ctx->timing.h2d_ms = ms(ctx->ev[0], ctx->ev[1]);
-    ctx->timing.front_ms = front_end;
-    ctx->timing.detect_ms = detect_end - detect_begin;
-    ctx->timing.total_ms = ms(ctx->ev[0], ctx->ev[3]);
-    ctx->timing.mixed_order_ms = ms(ctx->ev_t[0], ctx->ev_t[1]);
-    ctx->timing.mixed_classes = n_classes;
-    ctx->timing.detect_launches = ctx->timing.front_launches = (uint32_t)n_launch;
+    ctx->timing.mixed_classes = m.n_classes;
+    ctx->timing.front_launches = ctx->timing.detect_launches;
     ctx->timing.front_redone = cnt.front_redone;
     ctx->timing.front_repairs = cnt.front_repairs;
     ctx->timing.idle_skipped = cnt.idle_skipped;
     ctx->timing.idle_rewalks = cnt.idle_rewalks;
     ctx->timing.chain_folds = cnt.chain_folds;
     ctx->timing.chain_fm_rebuilds = cnt.chain_fm_rebuilds;
-    ctx->n_samples = n_samples;
+    ctx->n_samples = m.n_samples;
     ctx->processed = true;
-    return chain_finish(ctx, ch, last, settings, slots, true);
+    return chain_finish(ctx, ch, last, m.settings, m.slots, true);
 }
 
 } // namespace

@@ -432,8 +432,9 @@ class Context:
         self._check(self.L.r433b_set_pipeline(self.h, groups))
 
     def set_split(self, segment_blocks, warmup_blocks=1):
-        """Segmented replay of long streams (include/r433b.h: r433b_set_split): segment_blocks 0 = off, SPLIT_AUTO =
-        chosen from the batch.  Results are those of the unsplit batch."""
+        """Segmented replay of long streams (include/r433b.h: r433b_set_split) in process() and unchained
+        process_mixed(): segment_blocks 0 = off, SPLIT_AUTO = chosen from the batch.  Results are those of the unsplit
+        batch."""
         self._check(self.L.r433b_set_split(self.h, segment_blocks, warmup_blocks))
 
     def set_devices(self, devs):
@@ -510,7 +511,8 @@ class Context:
         """A batch whose stream i has its own sample format, rate and centre frequency (formats[i], rates[i], freqs[i];
         include/r433b.h: r433b_process_mixed).  `data`: host numpy array or an int device pointer.  With a Chain, stream
         i is the next chunk of slot i's file and `last[i]` says whether the file ends with it
-        (r433b_process_mixed_chained)."""
+        (r433b_process_mixed_chained).  Without a chain, set_split() splits the batch's long streams, every class in
+        the same passes; a chain runs unsplit."""
         offs = np.ascontiguousarray(offsets, dtype=np.uint64)
         n = len(offs) - 1
         if not (len(formats) == len(rates) == len(freqs) == n):
